@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the ElasticFusion hot path (track + fuse + predict) on B200, with the ICP-reduction roofline.
+"""bench.py — frames/sec of the ElasticFusion hot path (track + fuse + predict) on H100, with the ICP-reduction roofline.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload ...]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload ...] [--dump-outputs DIR]
 
 A *step* is one ElasticFusion::processFrame call on one frame of the synthetic ICL-NUIM-shaped room sequence; every rank (one
 per GPU) tracks and fuses its own independent sequence, so `value` is the whole-job frames/sec (weak scaling, no data-path
@@ -15,13 +15,23 @@ collective; NCCL only for the two barriers and the max-over-ranks, through elast
              inside the timed (wall-clock) region -- what a caller of libefusion.so sees.
   no_lookahead  both numbers with plain per-frame calls (the caller does not own frame i+1 while frame i runs).
   roofline   the ICP residual + Jacobian + 29-term reduction at level 0 (north_star's kernel): algorithmic 48 B/pixel + 116 B,
-             average launch duration over a batch of launches whose inputs exceed L2, against MEASURED_PEAKS.json hbm_gbs;
+             average launch duration over a batch of launches whose inputs exceed L2, against the HBM bandwidth peak (MEASURED_PEAKS.json
+             hbm_gbs when present, else the H100 SXM data-sheet figure);
              `full_iteration` is the complete Gauss-Newton iteration (k_iter1 + k_iter2) on the same bytes.
   value_1280x960, large_map   (rank 0, N=1 only) BASELINE configs[2] frames/sec, and frames/sec + per-pass GB/s with 5 M (640x480)
              and 20 M (1280x960) surfels RESIDENT: the map is pre-populated through ef_map_upload after the first frame.
   tracking_only  event-timed tracking stages of this library vs the reference's own CUDA tracking kernels (oracle/_ref) per frame.
   cpu_baseline   the reference arm on a bounded sample (reference CUDA tracking + CPU-oracle mapping; pure CPU port if oracle/_ref
              is absent).
+  gpu        name and power limit of the device the numbers were measured on.
+
+--dump-outputs DIR writes what the timed path computed in its last step, as a caller of ef_process_frame_device would read it:
+the camera pose, the model views predicted for the next frame (vertex, normal, colour; above 640x480 a fixed, seeded sample of
+307200 pixels) and a sample of the surfel map chosen and ordered by a hash of each surfel's quantised position, so that it does
+not depend on the order the map was written in or shift when another surfel is added or removed. At most 64 MB in all. Every file is
+finite: the map sample and the vertex and normal views hold 0 where the output holds NaN (an invalid entry), and
+<name>_nonfinite.npy marks those elements. The frames are a
+function of the workload and the sequence seed only, so two builds run with the same arguments can be compared output for output.
 
 --impl reference times the reference arm alone: the reference's CUDA tracking kernels compiled unmodified into oracle/_ref (driven
 launch-for-launch like Core/Utils/RGBDOdometry.cpp) plus the CPU oracle for the GLSL mapping half, which cannot run without OpenGL
@@ -36,6 +46,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -61,7 +72,7 @@ WORKLOADS = {
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling of SM clocks and throttle reasons during the timed region."""
 
     def __init__(self, device_index: int):
         self.idx = device_index
@@ -104,6 +115,76 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+MAP_SAMPLE = 200_000  # at most this many surfel rows kept by --dump-outputs (48 B each)
+VIEW_SAMPLE = 640 * 480  # at most this many pixels kept of each model view (16 B each)
+DUMP_LIMIT = 64 * 2 ** 20
+
+
+def position_hash(m):
+    """64-bit hash of each surfel's position quantised to 1 mm: a surfel hashes alike in two builds wherever the map stores it."""
+    xyz = np.nan_to_num(m[:, :3].astype(np.float64), nan=0.0, posinf=0.0, neginf=0.0)
+    q = np.round(xyz * 1000.0).astype(np.int64).view(np.uint64)
+    h = np.full(len(m), 0x9E3779B97F4A7C15, np.uint64)
+    for k in range(3):  # splitmix64-style mixing of the three coordinates
+        h = (h ^ q[:, k]) * np.uint64(0xBF58476D1CE4E5B9)
+        h ^= h >> np.uint64(31)
+    return h
+
+
+def map_sample(m):
+    """The surfels whose position hash is 0 modulo the smallest power of two that leaves at most MAP_SAMPLE of them, ordered by
+    hash. Which surfels are kept depends on their positions only, so two builds whose maps differ by a few surfels still keep
+    (almost) the same rows in the same order."""
+    h = position_hash(m)
+    k = 1
+    while np.count_nonzero(h % np.uint64(k) == 0) > MAP_SAMPLE:
+        k *= 2
+    keep = np.flatnonzero(h % np.uint64(k) == 0)
+    keep = keep[np.lexsort((m[keep, 2], m[keep, 1], m[keep, 0], h[keep]))]
+    return m[keep]
+
+
+def view_sample(a):
+    """A model view (H, W, C) whole when it has at most VIEW_SAMPLE pixels, else a fixed, seeded sample of VIEW_SAMPLE of its
+    pixels (row-major order, (VIEW_SAMPLE, C)); the sample depends on the resolution only."""
+    h, w = a.shape[:2]
+    if h * w <= VIEW_SAMPLE:
+        return a
+    idx = np.sort(np.random.default_rng(0).choice(h * w, VIEW_SAMPLE, replace=False))
+    return a.reshape(h * w, -1)[idx]
+
+
+def dump_outputs(ctx, pose, out_dir):
+    """The last timed step's outputs as out_dir/<name>.npy (float32 / float64, at most 64 MB in all at every workload)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"pose": pose.astype(np.float64), "map_count": np.array([ctx.map_count()], np.float64),
+              "map_sample": map_sample(ctx.map_download()).astype(np.float32)}
+    for name, buf in (("model_vertex", "VERTEX"), ("model_normal", "NORMAL"), ("model_image", "IMAGE")):
+        arrays[name] = view_sample(ctx.download(buf)).astype(np.float32)
+    # NaN marks invalid entries (e.g. the normal of a surfel at a depth edge): kept as a mask, written as 0 in the values
+    for name in ("map_sample", "model_vertex", "model_normal"):
+        bad = ~np.isfinite(arrays[name])
+        arrays[name + "_nonfinite"] = bad.astype(np.float32)
+        arrays[name] = np.where(bad, np.float32(0), arrays[name])
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, total
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def gpu_info(device_index):
+    """Name and power limit of the device (a measured number is only meaningful with both)."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(device_index), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        name, power = [c.strip() for c in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit": power}
+    except Exception:
+        import torch
+
+        return {"name": torch.cuda.get_device_name(device_index), "power_limit": None}
+
+
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -111,7 +192,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s)"
 
 
 def make_frames(K, n, seed):
@@ -119,7 +200,7 @@ def make_frames(K, n, seed):
     shorter request: the reference arm and repeated runs on one box do not render again)."""
     from elasticfusion_b200 import synth
 
-    cache = os.path.join(os.environ.get("EF_BENCH_CACHE", "/tmp"), f"ef_bench_{K.width}x{K.height}_{seed}.npz")
+    cache = os.path.join(os.environ.get("EF_BENCH_CACHE", tempfile.gettempdir()), f"ef_bench_{K.width}x{K.height}_{seed}.npz")
     have_rgb = have_depth = None
     if os.path.exists(cache):
         try:
@@ -260,7 +341,7 @@ def run_ours(args, rank, world, dist):
     la = not args.no_lookahead
     do_flush = not args.no_flush
     cfg = capi.default_config(K.width, K.height, K.fx, K.fy, K.cx, K.cy, capacity=cap, time_delta=BIG, device=local)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -288,6 +369,8 @@ def run_ours(args, rank, world, dist):
     dev_ms = float(sum(frame_ms))
     n_surfels = ctx.map_count()
     pose = ctx.get_pose()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ctx, pose, args.dump_outputs)
 
     # ---------------- roofline: ICP reduction at level 0, cold L2 ----------------
     roof = icp_roofline(ctx, stream, flush, K, rgb, depth, local)
@@ -345,7 +428,7 @@ def run_ours(args, rank, world, dist):
         "gpu_launches": int(round(launches)), "launches_per_frame": launches / args.steps,
         "clocks": clocks, "roofline": dict(roof, peak=hbm, frac=roof["achieved"] / hbm, peak_source=peak_src),
         "frame_ms": {"median": statistics.median(frame_ms), "p10": float(np.percentile(frame_ms, 10)), "p90": float(np.percentile(frame_ms, 90))},
-        "wall_s_value_loop": t_wall, "wall_fps_value_loop": args.steps / t_wall, "pose_check": float(np.abs(pose - pose2).max()),
+        "gpu": gpu_info(local), "wall_s_value_loop": t_wall, "wall_fps_value_loop": args.steps / t_wall, "pose_check": float(np.abs(pose - pose2).max()),
     }
     roof["full_iteration"]["frac"] = roof["full_iteration"]["achieved"] / hbm
     if nola:
@@ -479,7 +562,7 @@ def icp_roofline(ctx, stream, flush, K, rgb, depth, local):
     iteration of level 0) and of the complete iteration (k_iter1 + k_iter2: + final sums, 6x6 solve, pose update).
 
     cold (the HBM-roofline number): the launch is repeated round-robin over R independent contexts whose level-0 maps
-    together exceed the 126 MB L2 (R x 14.7 MB at 640x480, R x 59 MB at 1280x960), so every launch finds its inputs evicted;
+    together exceed the 50 MB L2 (R x 14.7 MB at 640x480, R x 59 MB at 1280x960), so every launch finds its inputs evicted;
     two CUDA events bracket the whole batch on the launching stream and the average per launch is reported -- inputs larger
     than L2, no flush inside the timed region, launch gaps included as in the frame loop. warm = the same batch on one
     context (L2 resident). single_launch_event_us = one launch between two events after a 256 MiB flush (adds the latency of
@@ -494,7 +577,7 @@ def icp_roofline(ctx, stream, flush, K, rgb, depth, local):
     ctx.icp_step_async(0, R, t, np.linalg.inv(R).astype(np.float32), t)
     ctx.sync()
     nbytes = 48 * K.width * K.height + 116
-    n_ctx = max(3, int(np.ceil(260e6 / nbytes)))  # level-0 maps in rotation: twice the 126 MB L2
+    n_ctx = max(3, int(np.ceil(100e6 / nbytes)))  # level-0 maps in rotation: twice the 50 MB L2
     cfg = capi.default_config(K.width, K.height, K.fx, K.fy, K.cx, K.cy, capacity=400_000 * (K.width // 640) ** 2, time_delta=BIG, device=local)
     ring = []
     for j in range(n_ctx):
@@ -543,17 +626,6 @@ def icp_roofline(ctx, stream, flush, K, rgb, depth, local):
 
     single_cold = single(lambda: ctx.icp_dense_pass_async(0))
     full_single = single(lambda: ctx.icp_step_async(0))
-    traffic = ncu_us = None
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        tp = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                traffic = tj.get(f"k_iter1_{K.width}x{K.height}")
-                ncu_us = tj.get(f"k_iter1_{K.width}x{K.height}_ncu_duration_us")
-                break
-            except Exception:
-                traffic = None
     return {"kernel": "k_iter1 (ICP residual + Jacobian + per-CTA 29-term reduction, level 0; ef_reduce.cu)", "bound": "hbm", "unit": "GB/s",
             "achieved": nbytes / (cold * 1e-6) / 1e9, "algorithmic_bytes": nbytes, "duration_us": cold,
             "achieved_warm_l2": nbytes / (warm * 1e-6) / 1e9, "duration_warm_us": warm,
@@ -561,10 +633,9 @@ def icp_roofline(ctx, stream, flush, K, rgb, depth, local):
             "full_iteration": {"kernels": "k_iter1 + k_iter2 (dense rows -> per-CTA partials -> final double sums -> 6x6 LDL^T -> pose update), ICP term only",
                                "algorithmic_bytes": nbytes, "duration_us": full_cold, "achieved": nbytes / (full_cold * 1e-6) / 1e9,
                                "duration_warm_us": full_warm, "single_launch_event_us": full_single, "unit": "GB/s"},
-            "traffic": traffic, "ncu_duration_us": ncu_us,
             "units_per_launch": f"{K.width * K.height} pixels (one Gauss-Newton iteration of pyramid level 0), 48 B each",
             "timing": (f"two CUDA events on the launching stream around a batch of 4 x {n_ctx} launches rotating over {n_ctx} contexts "
-                       f"({n_ctx * nbytes / 1e6:.0f} MB of level-0 maps, twice the 126 MB L2, so every launch is L2-cold), average per launch, median of 5 batches")}
+                       f"({n_ctx * nbytes / 1e6:.0f} MB of level-0 maps, at least twice the 50 MB L2, so every launch is L2-cold), average per launch, median of 5 batches")}
 
 
 def tracking_stage_ms(capi, stream, K, rgb, depth, local, cap, frames=40):
@@ -731,6 +802,7 @@ def main():
     ap.add_argument("--no-lookahead", action="store_true", help="process each frame without staging its successor on the side stream")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="headline numbers only: no 1280x960 / large-map / no-look-ahead extras")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Builds libefusion.so (the product: sm_100a CUDA kernels + C ABI) in-tree. No reference or oracle code is linked.
+# Builds libefusion.so (the product: sm_90a CUDA kernels + C ABI) in-tree. No reference or oracle code is linked.
 # Per-pixel kernels (image pyramids, map, preprocess) are compiled with --fmad=false so their results are bit-reproducible
 # against a plain C restatement; the reductions (ef_reduce.cu) keep FMA contraction like the reference build.
 set -e
@@ -8,7 +8,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 D=elasticfusion_b200/csrc
 B=build/obj
 mkdir -p $B
-COMMON="-std=c++17 -O3 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC,-O2,-Wall,-Wno-unknown-pragmas -ccbin /usr/bin/g++"
+COMMON="-std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC,-O2,-Wall,-Wno-unknown-pragmas -ccbin /usr/bin/g++"
 for f in ef_api ef_track ef_map ef_preprocess; do
   $NVCC $COMMON --fmad=false -c $D/$f.cu -o $B/$f.o "$@" &
 done

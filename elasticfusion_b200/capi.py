@@ -1,6 +1,6 @@
 """ctypes binding of libefusion.so (include/efusion_b200.h).
 
-This is the thinnest possible host layer: it loads the in-tree shared library that holds the sm_100a kernels and
+This is the thinnest possible host layer: it loads the in-tree shared library that holds the sm_90a kernels and
 calls its C ABI. There is no CPU fallback: if the library is missing or the call fails, an exception is raised.
 """
 from __future__ import annotations

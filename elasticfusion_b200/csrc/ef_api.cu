@@ -312,8 +312,7 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
     ctx->maps_dirty[0] = ctx->maps_dirty[1] = true;
     // Gauss-Newton iterations of the coarse pyramid levels inside one thread-block cluster (k_gn_cluster): EF_GN_CLUSTER = wanted
     // cluster size (16 default, 8, or 0 = off), EF_GN_CLUSTER_LEVELS = how many levels from the top of the pyramid (default 1: the 160x120
-    // level; measured 313 / 322 / 446 us for the whole loop with 1 / 2 / 3 levels against 338 without -- 16 SMs are too few for the
-    // dense pass of the finer levels)
+    // level; 16 SMs are too few for the dense pass of the finer levels)
     e = getenv("EF_VISIBLE_LIST");
     ctx->visible_list = !(e && e[0] == '0');
     ctx->vis_pending = false;

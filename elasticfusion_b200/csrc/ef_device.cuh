@@ -31,7 +31,7 @@ __host__ __device__ __forceinline__ f3 cross(const f3& a, const f3& b) {
 }
 __host__ __device__ __forceinline__ float dot(const f3& a, const f3& b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 __device__ __forceinline__ float norm(const f3& a) { return sqrtf(dot(a, a)); }
-// IEEE 1/sqrt (the reference's rsqrtf is the 2-ulp MUFU approximation; see DESIGN.md "numerics")
+// IEEE 1/sqrt (the reference's rsqrtf is the 2-ulp MUFU approximation)
 __device__ __forceinline__ f3 normalized(const f3& a) {
   const float rn = 1.0f / sqrtf(dot(a, a));
   return mk3(a.x * rn, a.y * rn, a.z * rn);

@@ -9,7 +9,7 @@ namespace ef {
 
 constexpr int NUM_PYRS = 3;          // RGBDOdometry::NUM_PYRS (reference Core/Utils/RGBDOdometry.h:114)
 constexpr int RED_THREADS = 256;     // threads per reduction CTA
-constexpr int MAX_RED_BLOCKS = 1184; // 148 SMs x 8 resident 256-thread CTAs
+constexpr int MAX_RED_BLOCKS = 1184; // 8 resident 256-thread CTAs per SM on up to 148 SMs (H100: 132)
 constexpr int PARTIAL_STRIDE = 64;   // floats per CTA partial: [0,29) geometric system, [32,61) photometric system
 constexpr int MAX_TRACE = 48;
 constexpr int MAX_RGB_BLOCKS = 160;

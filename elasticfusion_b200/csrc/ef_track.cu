@@ -1,15 +1,15 @@
 // Tracking half of the hot path: pyramid construction and the coarse-to-fine geometric + photometric
-// Gauss-Newton loop, as hand-written sm_100a kernels.
+// Gauss-Newton loop, as hand-written sm_90a kernels.
 //
 // Behavioural specification = the reference's Core/Cuda/{cudafuncs,reduce}.cu and Core/Utils/RGBDOdometry.cpp
-// (cited per kernel). Structure is B200-first rather than a translation:
+// (cited per kernel). Structure is GPU-first rather than a translation:
 //   * every reduction is ONE launch: per-CTA warp-shuffle tree -> per-CTA partial in HBM/L2 -> the CTA that takes
 //     the last ticket sums the partials in double and finishes the job (the reference uses 64 CTAs + a second
 //     1-CTA kernel + cudaDeviceSynchronize + a blocking D2H per step, reduce.cu:378-386);
 //   * the 6x6 / 3x3 solves, the SE(3) update and the next iteration's warp matrices are computed by that last
 //     CTA, so the whole SO(3) + 19-iteration SE(3) schedule is a stream of launches with no host round trip;
 //   * geometric and photometric systems of one iteration are reduced by the same launch;
-//   * grids are sized from the SM count (148 on B200), not the reference's fixed 64 CTAs (types.cuh:64-65);
+//   * grids are sized from the SM count (132 on H100), not the reference's fixed 64 CTAs (types.cuh:64-65);
 //   * the back-projected point cloud is recomputed in the photometric step instead of being stored.
 #include <float.h>
 #include <stddef.h>

@@ -388,7 +388,7 @@ class ElasticFusion {
   }
   void predict() { ef::check(ef_predict(ctx_), "predict"); }
 
-  // B200 additions for closed-loop hosts. The reference runs its CPU deformation solver in the middle of processFrame
+  // Additions for closed-loop hosts. The reference runs its CPU deformation solver in the middle of processFrame
   // (Core/ElasticFusion.cpp:505-526); a host that owns that solver splits the frame instead:
   //   processFrameBegin(...); c = getLocalLoopClosure(); <Deformation::constrain on c> ; processFrameEnd(&T_wc_est, graph, n)
   struct LocalLoopClosure {

@@ -10,7 +10,7 @@
 // hasMore() keeps the reference's "currentFrame + 1 < numFrames" (the last frame of a log is never delivered,
 // RawLogReader.cpp:139-141).
 //
-// B200 addition: peekNext() decodes the frame AFTER the current one into a second buffer pair without advancing, so the
+// Addition: peekNext() decodes the frame AFTER the current one into a second buffer pair without advancing, so the
 // caller can hand it to ElasticFusion::processFrame(..., nextRgb, nextDepth) for the look-ahead; the following getNext()
 // just flips the buffers.
 #ifndef EFUSION_B200_RAWLOGREADER_H_

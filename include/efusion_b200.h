@@ -1,4 +1,4 @@
-/* efusion_b200.h — C ABI of libefusion.so, the B200-native (sm_100a) implementation of ElasticFusion's per-frame
+/* efusion_b200.h — C ABI of libefusion.so, the H100-native (sm_90a) implementation of ElasticFusion's per-frame
  * tracking + surfel fuse/predict hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b): plain pointers and sizes, no C++/torch types. Each entry point

@@ -7,7 +7,7 @@
  *
  * PARITY PIN STATUS: the reference ships no tests, golden vectors or fixtures (SURVEY.md §4).
  *  - tracking half: pinned against the reference's own CUDA kernels compiled unmodified
- *    from /root/reference into oracle/_ref/ (run on the GPU box; tests/test_ref_pin.py).
+ *    from the reference tree into oracle/_ref/ (run on the GPU; tests/test_gpu_ref_pin.py).
  *  - mapping half (GLSL): pinned against the reference's own shader files, executed unmodified
  *    on Mesa 18 llvmpipe (the software libGL bundled with Nsight Compute in this image) by
  *    oracle/gl/ref_gl_harness.cpp; the outputs are committed as tests/golden/ref_mapping_160x120.npz

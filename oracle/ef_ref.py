@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY — ctypes binding for oracle/_ref/libef_ref.so: the REFERENCE's own CUDA tracking kernels
-(Core/Cuda/reduce.cu, cudafuncs.cu compiled unmodified from /root/reference) behind oracle/ref_harness.cu.
+(Core/Cuda/reduce.cu, cudafuncs.cu compiled unmodified from the reference tree) behind oracle/ref_harness.cu.
 Needs a GPU. Used to pin the CPU oracle and as the timed tracking baseline (bench.py --impl reference)."""
 from __future__ import annotations
 

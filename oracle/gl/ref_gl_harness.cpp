@@ -739,7 +739,7 @@ void efg_fill_image(const uint8_t* existing4, const uint8_t* rgb, int passthroug
 
 // ---- Resize::image / vertex / time (Resize.cpp:50-159): empty.vert + quad.geom + resize.frag into a (W/factor) x (H/factor)
 // target. which: 0 = RGBA8 image (read back as RGB, 3 bytes per texel), 1 = RGBA32F, 2 = R16UI through the float sampler
-// (formally undefined, see the note in DESIGN.md; reported as read back) ----
+// (formally undefined; reported as read back) ----
 static GLuint g_pResize = 0;
 void efg_resize(const void* src, int which, int factor, void* out) {
   if (!g_pResize) g_pResize = program("empty.vert", "resize.frag", "quad.geom", false);

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — harness around the REFERENCE's own CUDA tracking half.
 //
 // Built by oracle/Makefile (target `ref`) together with the reference's Core/Cuda/reduce.cu, cudafuncs.cu and
-// containers/device_memory.cpp, compiled UNMODIFIED from /root/reference for sm_100a, into oracle/_ref/libef_ref.so.
+// containers/device_memory.cpp, compiled UNMODIFIED from the reference tree for sm_90a, into oracle/_ref/libef_ref.so.
 // Purpose: (1) pin the CPU oracle against the real reference kernels on the GPU box, (2) time the reference's
 // tracking path exactly as the reference drives it (two launches + cudaDeviceSynchronize + blocking D2H per step).
 //

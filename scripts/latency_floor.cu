@@ -2,7 +2,7 @@
 // threads perform D dependent rounds of memory reads (D = 0: launch / drain only; 1: one round trip; 2, 3: the state -> live maps
 // -> gather chain), warm (L2 resident) and cold (a 512 MB working set rotated so every round misses L2), followed by the block
 // reduction + partial store k_iter1 ends with. Prints microseconds per launch (CUDA events around 200 chained launches).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o build/latency_floor scripts/latency_floor.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o build/latency_floor scripts/latency_floor.cu
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -1,4 +1,4 @@
-// The reference README's "How do I just use the Core API?" program (README.md:74-100), against libefusion.so (B200).
+// The reference README's "How do I just use the Core API?" program (README.md:74-100), against libefusion.so.
 // Usage: core_api_example <raw.klg> <width> <height> <fx> <fy> <cx> <cy> [lookahead]  -> prints the final pose and surfel
 // count. With `lookahead` the log is read one frame ahead and the next frame is handed to processFrame as well.
 #include <ElasticFusion.h>

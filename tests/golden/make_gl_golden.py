@@ -1,9 +1,10 @@
-"""Generates tests/golden/ref_mapping_160x120.npz: the inputs and outputs of every GLSL pass of the reference's mapping half,
-produced by the REFERENCE's OWN SHADER FILES (/root/reference/Core/Shaders, unmodified) executed on Mesa llvmpipe through
-oracle/gl/ref_gl_harness.cpp (`make -C oracle refgl`). Run in the build container:  python tests/golden/make_gl_golden.py
+"""Generates tests/golden/ref_mapping_160x120.npz: the outputs of every GLSL pass of the reference's mapping half, produced by
+the REFERENCE's OWN SHADER FILES (Core/Shaders of the reference tree, unmodified) executed on Mesa llvmpipe through
+oracle/gl/ref_gl_harness.cpp (`make -C oracle refgl`, which needs the reference tree):  python tests/golden/make_gl_golden.py
 
 The chain of inputs is the one a frame goes through (the stage outputs of the CPU oracle feed the next stage on both sides, so
-every pass is compared on identical inputs); `gl_*` arrays are what the reference's shaders computed."""
+every pass is compared on identical inputs; tests/test_gl_golden.py:oracle_inputs recomputes them); `gl_*` arrays are what the
+reference's shaders computed, the large ones cut to a regular sample (test_gl_golden.shrink)."""
 import os
 import sys
 
@@ -23,32 +24,15 @@ if not rg.in_gl_process():
 
 from elasticfusion_b200 import synth  # noqa: E402
 from oracle import ef_oracle as eo  # noqa: E402
-from util import run_oracle  # noqa: E402
+import test_gl_golden as tg  # noqa: E402
 
 MAXD, BIG = 20.0, 2 ** 30
 
 
-def graph_for(m, n_nodes=40, seed=4):
-    rng = np.random.RandomState(seed)
-    idx = np.sort(rng.choice(len(m), n_nodes, replace=False))
-    nodes = np.zeros((n_nodes, 16), np.float32)
-    for k, i in enumerate(idx):
-        w = rng.standard_normal(3) * 0.01
-        th = np.linalg.norm(w)
-        kx = np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]]) / max(th, 1e-12)
-        R = np.eye(3) + np.sin(th) * kx + (1 - np.cos(th)) * (kx @ kx)
-        nodes[k, 0:3] = m[i, 0:3]
-        nodes[k, 3:12] = R.T.reshape(-1)
-        nodes[k, 12:15] = rng.standard_normal(3) * 0.01
-        nodes[k, 15] = m[i, 6]
-    return np.ascontiguousarray(nodes[np.argsort(nodes[:, 15], kind="stable")])
-
-
 CONFIGS = {
-    # the committed fixture
     "default": dict(K=(160, 120, 132.0, 132.0, 80.0, 60.0), seed=7, speed=1.0),
-    # live checks only (tests/test_gl_golden.py::test_oracle_matches_reference_shaders_live): the ICL-NUIM camera (fx != fy, half-pixel
-    # principal point; SURVEY 8d S1) at a quarter of its resolution, and an off-centre camera with another aspect ratio
+    # the ICL-NUIM camera (fx != fy, half-pixel principal point; SURVEY 8d S1) at a quarter and at half of its resolution, and an
+    # off-centre camera with another aspect ratio
     "icl": dict(K=(160, 120, 481.2 / 4, 480.0 / 4, 319.5 / 4, 239.5 / 4), seed=11, speed=1.0),
     "offcentre": dict(K=(192, 144, 150.0, 155.0, 90.3, 70.7), seed=23, speed=2.0),
     "icl320": dict(K=(320, 240, 481.2 / 2, 480.0 / 2, 319.5 / 2, 239.5 / 2), seed=5, speed=1.5),
@@ -56,93 +40,70 @@ CONFIGS = {
 
 
 def build(config="default"):
-    """Inputs and the reference shaders' outputs of every pass for one configuration (a dict of arrays)."""
+    """The reference shaders' outputs of every pass for one configuration, and the inputs they were given (a dict of arrays)."""
     cfg = CONFIGS[config]
     K = synth.Intrinsics(int(cfg["K"][0]), int(cfg["K"][1]), *[float(x) for x in cfg["K"][2:]])
-    frames = list(synth.sequence(8, K, seed=cfg["seed"], noise=True, speed=cfg["speed"]))
+    g = tg.oracle_inputs(K, cfg["seed"], cfg["speed"])
     gl = rg.RefGL(K)
-    out = {"K": np.array([K.width, K.height, K.fx, K.fy, K.cx, K.cy], np.float64), "gl_log": np.array(gl.log())}
+    out = {"K": np.array([K.width, K.height, K.fx, K.fy, K.cx, K.cy], np.float64), "seed": np.array(cfg["seed"]), "speed": np.array(cfg["speed"]),
+           "gl_log": np.array(gl.log())}
+    T, tick, tick_t, td = g["T"], int(g["tick"]), int(g["tick_t"]), int(g["td"])
     # ---- frame 0: preprocess + first-frame map
-    rgb0, depth0, _ = frames[0]
-    out.update(rgb0=rgb0, depth0=depth0, gl_bilateral=gl.bilateral(depth0, 3.0), gl_metric=gl.metric(depth0, 3.0))
-    filt0 = eo.bilateral(depth0, 3.0)
-    dm0, dmf0 = eo.metric(depth0, 3.0), eo.metric(filt0, 3.0)
-    out.update(filt0=filt0, gl_metric_filtered=gl.metric(filt0, 3.0))
-    raw, fil = gl.feedback_buffer(rgb0, dm0, 1, MAXD), gl.feedback_buffer(rgb0, dmf0, 1, MAXD)
-    out.update(gl_feedback_raw=raw, gl_feedback_filt=fil, gl_initial_map=gl.map_initialise(raw, fil))
-    # a scene crossing depthCutoff: the two feedback buffers differ in length (SURVEY App. A-29)
-    Tb = synth.pose(synth.rot_xyz(0, np.deg2rad(55.0), 0), [-1.6, 0.2, -1.2])
-    rgbb, depthb, _, _ = synth.render(Tb, K, noise_seed=77)
-    filtb = eo.bilateral(depthb, 3.0)
-    rawb, filb = gl.feedback_buffer(rgbb, eo.metric(depthb, 3.0), 1, MAXD), gl.feedback_buffer(rgbb, eo.metric(filtb, 3.0), 1, MAXD)
-    out.update(rgbb=rgbb, depthb=depthb, filtb=filtb, gl_boundary_raw_count=np.array(len(rawb)), gl_boundary_filt_count=np.array(len(filb)),
-               gl_boundary_map=gl.map_initialise(rawb, filb))
-    # ---- a map after 4 frames, frame 4 as the measurement
-    f = run_oracle(frames, K, 4)
-    m, T, tick = f.map(), f.pose, f.tick
-    rgb4, depth4, _ = frames[4]
-    filt4 = eo.bilateral(depth4, 3.0)
-    dm4, dmf4 = eo.metric(depth4, 3.0), eo.metric(filt4, 3.0)
-    out.update(map=m, T=T, tick=np.array(tick), rgb4=rgb4, depth4=depth4, filt4=filt4)
+    out.update(gl_bilateral=gl.bilateral(g["depth0"], 3.0), gl_metric=gl.metric(g["depth0"], 3.0))
+    raw = gl.feedback_buffer(g["rgb0"], eo.metric(g["depth0"], 3.0), 1, MAXD)
+    fil = gl.feedback_buffer(g["rgb0"], eo.metric(g["filt0"], 3.0), 1, MAXD)
+    out.update(gl_initial_map=gl.map_initialise(raw, fil))
+    rawb = gl.feedback_buffer(g["rgbb"], eo.metric(g["depthb"], 3.0), 1, MAXD)
+    filb = gl.feedback_buffer(g["rgbb"], eo.metric(g["filtb"], 3.0), 1, MAXD)
+    out.update(gl_boundary_raw_count=np.array(len(rawb)), gl_boundary_filt_count=np.array(len(filb)), gl_boundary_map=gl.map_initialise(rawb, filb))
+    # ---- the map after 4 frames, frame 4 as the measurement
+    m = g["map"]
     ig = gl.predict_indices(m, T, tick, MAXD, BIG)
     out.update(gl_index=ig[0], gl_vert_conf=ig[1], gl_color_time=ig[2], gl_norm_rad=ig[3])
-    io = eo.predict_indices(m, T, tick, MAXD, BIG, K)  # the chain continues on the oracle's index map (both sides use it)
-    out.update(index_in=io[0], vert_conf_in=io[1], color_time_in=io[2], norm_rad_in=io[3])
-    fused_gl, new_gl = gl.fuse(m, T, tick, rgb4, dm4, dmf4, *io, MAXD, 0.73)
+    io = (g["index_in"], g["vert_conf_in"], g["color_time_in"], g["norm_rad_in"])
+    fused_gl, new_gl = gl.fuse(m, T, tick, g["rgb4"], eo.metric(g["depth4"], 3.0), eo.metric(g["filt4"], 3.0), *io, MAXD, 0.73)
     out.update(gl_fused=fused_gl, gl_fuse_feedback=new_gl)
-    fused, new = eo.fuse(m, T, tick, rgb4, dm4, dmf4, *io, MAXD, 0.73, K)
-    io2 = eo.predict_indices(fused, T, tick, MAXD, BIG, K)
-    out.update(fused_in=fused, new_in=new, index2_in=io2[0], vert_conf2_in=io2[1], color_time2_in=io2[2], norm_rad2_in=io2[3])
-    out.update(gl_cleaned=gl.clean(fused, new_gl, T, tick, *io2, 10.0, BIG, MAXD))
-    # finite time window + un-cull branch: a map with old time stamps
-    mt = fused.copy()
-    n = len(mt)
-    mt[:, 6] = 1 + np.floor(np.arange(n) * 50.0 / n)
-    mt[:, 7] = np.maximum(np.where(np.arange(n) % 2 == 0, 20.0, 58.0), mt[:, 6])
-    mt[:, 3] += np.where(np.arange(n) % 3 == 0, 10.0, 0.0).astype(np.float32)
-    tick_t, td = 60, 8
-    it = eo.predict_indices(mt, T, tick_t, MAXD, td, K)
-    igt = gl.predict_indices(mt, T, tick_t, MAXD, td)
-    out.update(map_t=mt, tick_t=np.array(tick_t), td=np.array(td), gl_index_t=igt[0], index_t_in=it[0], vert_conf_t_in=it[1], color_time_t_in=it[2],
-               norm_rad_t_in=it[3])
+    io2 = (g["index2_in"], g["vert_conf2_in"], g["color_time2_in"], g["norm_rad2_in"])
+    out.update(gl_cleaned=gl.clean(g["fused_in"], new_gl, T, tick, *io2, 10.0, BIG, MAXD))
+    mt = g["map_t"]
+    it = (g["index_t_in"], g["vert_conf_t_in"], g["color_time_t_in"], g["norm_rad_t_in"])
+    out.update(gl_index_t=gl.predict_indices(mt, T, tick_t, MAXD, td)[0])
     none = np.zeros((0, 12), np.float32)
     out.update(gl_cleaned_t=gl.clean(mt, none, T, tick_t, *it, 10.0, td, MAXD))
-    # deformation graph inside clean (copy_unstable.vert:132-322)
-    nodes = graph_for(mt)
-    depth_t_gl = gl.combined_predict(mt, T, MAXD, 10.0, tick_t, tick_t - td, 65535, depth_only=True)
-    depth_t = eo.combined_predict(mt, T, MAXD, 10.0, tick_t, tick_t - td, 65535, K, depth_only=True)
-    out.update(nodes=nodes, gl_synth_depth_t=depth_t_gl, synth_depth_t_in=depth_t,
-               gl_cleaned_deformed=gl.clean(mt, none, T, tick_t, *it, 10.0, td, MAXD, nodes=nodes, depth=depth_t))
+    out.update(gl_cleaned_deformed=gl.clean(mt, none, T, tick_t, *it, 10.0, td, MAXD, nodes=g["nodes"], depth=g["synth_depth_t_in"]))
     # ---- model raycast (ACTIVE, INACTIVE, depth) and fill-in
-    ms = fused.copy()
-    ms[:, 3] += 10.0
+    ms = g["map_stable"]
     pg = gl.combined_predict(ms, T, MAXD, 10.0, tick, tick, BIG)
-    out.update(map_stable=ms, gl_image=pg[0], gl_vertex=pg[1], gl_normal=pg[2], gl_time=pg[3],
+    out.update(gl_image=pg[0], gl_vertex=pg[1], gl_normal=pg[2], gl_time=pg[3],
                gl_synth_depth=gl.combined_predict(ms, T, MAXD, 10.0, tick, tick, BIG, depth_only=True))
     pin = gl.combined_predict(mt, T, MAXD, 10.0, 0, tick_t - td, td)
     out.update(gl_old_image=pin[0], gl_old_vertex=pin[1], gl_old_normal=pin[2], gl_old_time=pin[3])
-    po = eo.combined_predict(ms, T, MAXD, 10.0, tick, tick, BIG, K)
-    out.update(image_in=po[0], vertex_in=po[1], normal_in=po[2])
-    out.update(gl_fill_vertex=gl.fill_vertex(po[1], filt4, 0), gl_fill_normal=gl.fill_normal(po[2], filt4, 0), gl_fill_image=gl.fill_image(po[0], rgb4, 0),
-               gl_fill_vertex_pass=gl.fill_vertex(po[1], filt4, 1), gl_fill_image_pass=gl.fill_image(po[0], rgb4, 1))
+    vi, ni, ii, filt4, rgb4 = g["vertex_in"], g["normal_in"], g["image_in"], g["filt4"], g["rgb4"]
+    out.update(gl_fill_vertex=gl.fill_vertex(vi, filt4, 0), gl_fill_normal=gl.fill_normal(ni, filt4, 0), gl_fill_image=gl.fill_image(ii, rgb4, 0),
+               gl_fill_vertex_pass=gl.fill_vertex(vi, filt4, 1), gl_fill_image_pass=gl.fill_image(ii, rgb4, 1))
     out["gl_error"] = np.array(int(gl.lib.efg_gl_error()))
-    return out, K
+    return out, g, K
 
 
 def main():
     if len(sys.argv) > 2 and sys.argv[1] == "--check":
         # live pin of the oracle in another configuration: nothing is written; the oracle is compared with what the shaders just
         # produced, with the same pass-by-pass checks the fixture test applies
-        import test_gl_golden as tg
-
-        out, K = build(sys.argv[2])
+        out, g, K = build(sys.argv[2])
         assert int(out["gl_error"]) == 0 and "llvmpipe" in str(out["gl_log"])
-        tg.run_all(tg.Oracle(K), out, K, False)
+        tg.run_all(tg.Oracle(K), dict(g, **out), K, False)
         print("LIVE OK", sys.argv[2])
         return
-    out, _ = build("default")
-    path = os.path.join(ROOT, "tests", "golden", "ref_mapping_160x120.npz")
-    np.savez_compressed(path, **out)
+    if len(sys.argv) == 1:  # one process per configuration: the GL harness keeps the frame size of its first context
+        import subprocess
+
+        for config in tg.FIXTURES:
+            subprocess.check_call([sys.executable, os.path.abspath(__file__), config])
+        return
+    config = sys.argv[1]
+    out, _, _ = build(config)
+    path = tg.fixture_path(config)
+    np.savez_compressed(path, **tg.shrink(out, tg.FIXTURES[config]))
     print("wrote", path, os.path.getsize(path) // 1024, "KiB; gl error", int(out["gl_error"]))
     print(out["gl_log"])
 

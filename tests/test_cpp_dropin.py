@@ -22,15 +22,6 @@ def test_core_api_example_compiles(tmp_path):
     _compile(str(tmp_path / "example"))
 
 
-def test_core_api_example_compiles_with_reference_sophus(tmp_path):
-    """With the reference's vendored Sophus + Eigen on the include path the pose type is Sophus::SE3d, as in the reference."""
-    ref = "/root/reference/third-party"
-    if not os.path.isdir(os.path.join(ref, "Sophus")):
-        pytest.skip("reference tree not present (GPU box)")
-    subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-fsyntax-only", "-DEIGEN_MAX_ALIGN_BYTES=0", f"-I{ref}/Sophus", f"-I{ref}/Eigen",
-                           f"-I{ROOT}/include/efusion", f"-I{ROOT}/include", SRC])
-
-
 @pytest.mark.gpu
 def test_core_api_example_runs_and_matches_c_abi(tmp_path, small_K, small_frames):
     from elasticfusion_b200 import capi, synth

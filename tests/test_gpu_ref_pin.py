@@ -1,5 +1,5 @@
 """Pins the CPU oracle's tracking half against the REFERENCE's own CUDA kernels (oracle/_ref/libef_ref.so: reduce.cu and
-cudafuncs.cu compiled unmodified from the reference tree, run on the GPU box) and checks the product against the same
+cudafuncs.cu compiled unmodified from the reference tree, run on the GPU) and checks the product against the same
 reference outputs. Tolerances cover what legitimately differs: nvcc's FMA contraction and approximate rsqrtf in the
 reference build vs single IEEE ops in oracle/product, and reduction order."""
 import numpy as np
