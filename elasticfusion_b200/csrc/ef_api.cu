@@ -190,7 +190,8 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   CU(A->alloc(&od.gn, 1));
   od.cand_base = reinterpret_cast<const int*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, cand_base));
   CU(A->alloc(&od.so3s, 1));
-  CU(A->alloc(&od.so3_partials, (size_t)MAX_RGB_BLOCKS * PARTIAL_STRIDE));
+  // one slot per CTA of k_so3_step, whose grid red_blocks() caps at MAX_RED_BLOCKS (254 CTAs at 1920x1080 on an H100)
+  CU(A->alloc(&od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE));
   CU(A->alloc(&od.so3_counter, 4));
   CU(cudaMemsetAsync(od.so3s, 0, sizeof(So3State), ctx->stream));
   CU(cudaMemsetAsync(od.so3_counter, 0, 16, ctx->stream));
@@ -199,7 +200,7 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   CU(A->alloc(&od.partials2, (size_t)MAX_RGB_BLOCKS * 32));
   // (the reductions read whole 32-float rows of these; the kernels write the 29 / 11 terms of a system, so the padding lanes
   // are defined once here)
-  CU(cudaMemsetAsync(od.so3_partials, 0, (size_t)MAX_RGB_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream));
+  CU(cudaMemsetAsync(od.so3_partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream));
   CU(cudaMemsetAsync(od.partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream));
   CU(cudaMemsetAsync(od.partials_rgb, 0, (size_t)MAX_RGB_BLOCKS * 32 * sizeof(float), ctx->stream));
   CU(cudaMemsetAsync(od.partials2, 0, (size_t)MAX_RGB_BLOCKS * 32 * sizeof(double), ctx->stream));
@@ -257,6 +258,7 @@ cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n) {
 }
 template cudaError_t ctx_alloc<float4>(EfContext*, float4**, size_t);
 template cudaError_t ctx_alloc<float>(EfContext*, float**, size_t);
+template cudaError_t ctx_alloc<double>(EfContext*, double**, size_t);
 template cudaError_t ctx_alloc<int>(EfContext*, int**, size_t);
 template cudaError_t ctx_alloc<unsigned int>(EfContext*, unsigned int**, size_t);
 template cudaError_t ctx_alloc<unsigned long long>(EfContext*, unsigned long long**, size_t);
@@ -402,9 +404,9 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
       }
     }
     TA(la.so3s, 1);
-    TA(la.so3_partials, (size_t)MAX_RGB_BLOCKS * PARTIAL_STRIDE);
+    TA(la.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE);
     TA(la.so3_counter, 4);
-    if (!rc) cudaMemsetAsync(la.so3_partials, 0, (size_t)MAX_RGB_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream);
+    if (!rc) cudaMemsetAsync(la.so3_partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream);
     if (!rc) {
       cudaError_t e = cudaStreamCreateWithFlags(&la.stream, cudaStreamNonBlocking);
       if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.ready, cudaEventDisableTiming);
@@ -1191,15 +1193,9 @@ extern "C" int ef_process_frame_end(EfContext* ctx, const double* T_wc_override,
 extern "C" int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* src3, double* dst3, int32_t* times, int32_t max_constraints,
                                     int32_t* n_out) {
   if (!ctx || !out || max_constraints < 0) return EF_EINVAL;
-  LoopDev* L = ctx->map.loop;
-  struct Head {
-    int ran, accepted, n_constraints;
-    float lastICPError, lastICPCount;
-    double cov_diag[6];
-    double T_wc_est[16];
-  } h;
-  static_assert(offsetof(LoopDev, src) >= sizeof(Head), "LoopDev header layout");
-  CU(cudaMemcpyAsync(&h, L, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  const MapDev& m = ctx->map;
+  LoopDev h;
+  CU(cudaMemcpyAsync(&h, m.loop, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   out->ran = h.ran;
   out->accepted = h.accepted;
@@ -1209,11 +1205,12 @@ extern "C" int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* s
   memcpy(out->cov_diag, h.cov_diag, sizeof(h.cov_diag));
   memcpy(out->T_wc_est, h.T_wc_est, sizeof(h.T_wc_est));
   int n = h.n_constraints < max_constraints ? h.n_constraints : max_constraints;
+  if (n > m.loop_capacity) n = m.loop_capacity;
   if (n_out) *n_out = n;
   if (n > 0) {
-    if (src3) CU(cudaMemcpyAsync(src3, (char*)L + offsetof(LoopDev, src), sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (dst3) CU(cudaMemcpyAsync(dst3, (char*)L + offsetof(LoopDev, dst), sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (times) CU(cudaMemcpyAsync(times, (char*)L + offsetof(LoopDev, times), sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (src3) CU(cudaMemcpyAsync(src3, m.loop_src, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (dst3) CU(cudaMemcpyAsync(dst3, m.loop_dst, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (times) CU(cudaMemcpyAsync(times, m.loop_times, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
   }
   return 0;

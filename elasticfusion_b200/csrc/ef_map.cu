@@ -1465,6 +1465,10 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &m.nodes, (size_t)MAX_GRAPH_NODES * 16));
   CU(ctx_alloc(ctx, &m.loop, 1));
   CU(cudaMemsetAsync(m.loop, 0, sizeof(LoopDev), ctx->stream));
+  m.loop_capacity = loop_constraint_capacity(c.width, c.height);
+  CU(ctx_alloc(ctx, &m.loop_src, (size_t)m.loop_capacity * 3));
+  CU(ctx_alloc(ctx, &m.loop_dst, (size_t)m.loop_capacity * 3));
+  CU(ctx_alloc(ctx, &m.loop_times, (size_t)m.loop_capacity));
   B->scan_epoch = 0;
   B->scan_state_bytes = tiles * 8;
   CU(cudaMemsetAsync(m.scan_tile_state, 0, tiles * 8, ctx->stream));
@@ -1793,11 +1797,14 @@ int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes) {
 }
 
 // ---- local loop closure front half, last step (ElasticFusion.cpp:473-505): acceptance test on the model-to-model result and
-// the constraint pairs sampled on the W/20 x H/20 grid (Resize::vertex / Resize::time = nearest sampling at texel centres)
+// the constraint pairs sampled on the W/20 x H/20 grid (Resize::vertex / Resize::time = nearest sampling at texel centres).
+// src / dst / times hold `capacity` constraints, one per grid cell; the bound check only guards against a caller that sized
+// them for another frame
 __global__ void __launch_bounds__(256) k_loop_constraints(const GNState* __restrict__ gn_curr, const GNState* __restrict__ gn_est,
                                                           const float4* __restrict__ vertex, const uint16_t* __restrict__ old_time, int rows,
                                                           int cols, float max_depth, int count_thresh, float err_thresh, float cov_thresh,
-                                                          LoopDev* out) {
+                                                          LoopDev* out, double* __restrict__ src, double* __restrict__ dst,
+                                                          int* __restrict__ times, int capacity) {
   pdl_enter();
   if (blockIdx.x != 0) return;
   __shared__ int s_accept, s_base, s_warp[8];
@@ -1842,15 +1849,15 @@ __global__ void __launch_bounds__(256) k_loop_constraints(const GNState* __restr
     __syncthreads();
     int off = s_base;
     for (int w = 0; w < wid; ++w) off += s_warp[w];
-    if (ok) {
-      const int o = off + __popc(b & ((1u << lane) - 1u));
+    const int o = off + __popc(b & ((1u << lane) - 1u));
+    if (ok && o < capacity) {
       const double x = v.x, y = v.y, z = v.z;
 #pragma unroll
       for (int r = 0; r < 3; ++r) {
-        out->src[o * 3 + r] = gn_curr->T_wc[r * 4 + 0] * x + gn_curr->T_wc[r * 4 + 1] * y + gn_curr->T_wc[r * 4 + 2] * z + gn_curr->T_wc[r * 4 + 3];
-        out->dst[o * 3 + r] = gn_est->T_wc[r * 4 + 0] * x + gn_est->T_wc[r * 4 + 1] * y + gn_est->T_wc[r * 4 + 2] * z + gn_est->T_wc[r * 4 + 3];
+        src[o * 3 + r] = gn_curr->T_wc[r * 4 + 0] * x + gn_curr->T_wc[r * 4 + 1] * y + gn_curr->T_wc[r * 4 + 2] * z + gn_curr->T_wc[r * 4 + 3];
+        dst[o * 3 + r] = gn_est->T_wc[r * 4 + 0] * x + gn_est->T_wc[r * 4 + 1] * y + gn_est->T_wc[r * 4 + 2] * z + gn_est->T_wc[r * 4 + 3];
       }
-      out->times[o] = t;
+      times[o] = t;
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -1860,7 +1867,7 @@ __global__ void __launch_bounds__(256) k_loop_constraints(const GNState* __restr
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) out->n_constraints = s_base;
+  if (threadIdx.x == 0) out->n_constraints = s_base < capacity ? s_base : capacity;
 }
 
 __global__ void k_loop_reset(LoopDev* out) {
@@ -1880,7 +1887,8 @@ __global__ void k_copy_pose(GNState* dst, const GNState* src) {
 int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh) {
   MapDev& m = ctx->map;
   EF_LAUNCH(ctx, k_loop_constraints, 1, 256, 0, (const GNState*)ctx->odom[0].gn, (const GNState*)ctx->odom[1].gn, (const float4*)ctx->tex.vertex,
-            (const uint16_t*)ctx->tex.old_time, m.rows, m.cols, ctx->max_depth_processed, count_thresh, err_thresh, cov_thresh, m.loop);
+            (const uint16_t*)ctx->tex.old_time, m.rows, m.cols, ctx->max_depth_processed, count_thresh, err_thresh, cov_thresh, m.loop,
+            m.loop_src, m.loop_dst, m.loop_times, m.loop_capacity);
   LAST();
   return 0;
 }
