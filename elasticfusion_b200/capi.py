@@ -34,6 +34,11 @@ class EfLoopResult(C.Structure):
                 ("lastICPCount", C.c_float), ("cov_diag", C.c_double * 6), ("T_wc_est", C.c_double * 16)]
 
 
+class EfDeformResult(C.Structure):
+    _fields_ = [("n_nodes", C.c_int32), ("n_enabled", C.c_int32), ("n_constraints", C.c_int32), ("iterations", C.c_int32),
+                ("stop", C.c_int32), ("bandwidth", C.c_int32), ("error", C.c_float), ("meanConsErr", C.c_float)]
+
+
 TRACE_DTYPE = np.dtype([
     ("kind", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("rgb_count", "<i4"), ("rgb_sigma", "<i4"),
     ("sigma_val", "<f4"),
@@ -223,6 +228,29 @@ class Context:
         info = dict(ran=res.ran, accepted=res.accepted, n_constraints=res.n_constraints, lastICPError=res.lastICPError,
                     lastICPCount=res.lastICPCount, cov_diag=np.array(res.cov_diag[:]), T_wc_est=np.array(res.T_wc_est[:]).reshape(4, 4))
         return info, src[:n.value].copy(), dst[:n.value].copy(), tm[:n.value].copy()
+
+    def deform_solve(self, node_pos, node_times, src, dst, src_times, dst_times=None, pin=False, last_deform_time=0):
+        """Local-loop-closure deformation solve (ef_deform_solve). Returns (info dict, nodes16 (n,16) float32,
+        constraint nodes (m,4) int32, constraint weights (m,4) float64, R (n,3,3) float64, t (n,3) float64); m counts the pin
+        constraints when pin is set."""
+        pos = np.ascontiguousarray(node_pos, np.float64).reshape(-1, 3)
+        nt = np.ascontiguousarray(node_times, np.int32)
+        s = np.ascontiguousarray(src, np.float64).reshape(-1, 3)
+        d = np.ascontiguousarray(dst, np.float64).reshape(-1, 3)
+        st = np.ascontiguousarray(src_times, np.int32)
+        dt = None if dst_times is None else np.ascontiguousarray(dst_times, np.int32)
+        n, nc = len(pos), len(s)
+        m = 2 * nc if pin else nc
+        nodes = np.zeros((max(n, 1), 16), np.float32)
+        cn = np.zeros((max(m, 1), 4), np.int32)
+        cw = np.zeros((max(m, 1), 4), np.float64)
+        rt = np.zeros((max(n, 1), 12), np.float64)
+        res = EfDeformResult()
+        _chk(lib().ef_deform_solve(self.h_ctx, _p(pos), _p(nt), n, _p(s), _p(d), _p(st), _p(dt), nc, int(pin), int(last_deform_time),
+                                   _p(nodes), _p(rt), _p(cn), _p(cw), C.byref(res)))
+        info = {k: getattr(res, k) for k, _ in EfDeformResult._fields_}
+        R = rt[:n, :9].reshape(n, 3, 3).transpose(0, 2, 1).copy()  # column-major -> R[i, row, col]
+        return info, nodes[:n], cn[:m], cw[:m], R, rt[:n, 9:].copy()
 
     def predict(self):
         _chk(lib().ef_predict(self.h_ctx))

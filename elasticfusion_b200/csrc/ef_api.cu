@@ -52,6 +52,11 @@ int map_dense_enough_async(EfContext* ctx);
 int map_tick_increment_async(EfContext* ctx);
 int map_select_model_inputs(EfContext* ctx, const float** vtx, const float** nrm, const uint8_t** img);
 void map_free_host(EfContext* ctx);
+
+int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
+                 const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
+                 int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out);
+void deform_free(EfContext* ctx);
 }  // namespace ef
 
 #define CU(x)                                  \
@@ -457,6 +462,7 @@ extern "C" int ef_destroy(EfContext* ctx) {
   if (ctx->la.pin_rgb) cudaFreeHost(ctx->la.pin_rgb);
   if (ctx->la.pin_depth) cudaFreeHost(ctx->la.pin_depth);
   map_free_host(ctx);
+  deform_free(ctx);
   for (void* p : arena(ctx)->blocks) cudaFree(p);
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
@@ -1214,6 +1220,35 @@ extern "C" int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* s
     CU(cudaStreamSynchronize(ctx->stream));
   }
   return 0;
+}
+
+// Deformation::constrain for a local loop closure (Deformation.cpp:73-207) on host inputs: constraints are expanded to
+// [c0, pin0, c1, pin1, ...] when `pin` is set (addConstraint, :73-86), then weighted, solved and handed over on the device.
+extern "C" int ef_deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int32_t n_nodes, const double* src3,
+                               const double* dst3, const int32_t* src_times, const int32_t* dst_times, int32_t n_constraints, int32_t pin,
+                               int32_t last_deform_time, float* nodes16, double* rt12, int32_t* cons_nodes4, double* cons_weights4,
+                               EfDeformResult* out) {
+  if (!ctx || !out || !node_pos3 || !node_times || !src3 || !dst3 || !src_times || (pin && !dst_times)) return EF_EINVAL;
+  if (n_nodes < 5 || n_nodes >= MAX_GRAPH_NODES || n_constraints < 1 || last_deform_time < 0) return EF_EINVAL;
+  for (int i = 0; i < n_nodes; ++i)  // the graph is sampled in time order (Deformation.cpp:294-296)
+    if (node_times[i] < 0 || (i > 0 && node_times[i] < node_times[i - 1])) return EF_EINVAL;
+  const int m = pin ? 2 * n_constraints : n_constraints;
+  std::vector<double> s(3 * (size_t)m), d(3 * (size_t)m);
+  std::vector<int32_t> t(m);
+  for (int i = 0, o = 0; i < n_constraints; ++i) {
+    if (src_times[i] < 0 || (pin && dst_times[i] < 0)) return EF_EINVAL;
+    memcpy(&s[3 * o], src3 + 3 * i, sizeof(double) * 3);
+    memcpy(&d[3 * o], dst3 + 3 * i, sizeof(double) * 3);
+    t[o++] = src_times[i];
+    if (pin) {  // (target, target, targetTime, targetTime)
+      memcpy(&s[3 * o], dst3 + 3 * i, sizeof(double) * 3);
+      memcpy(&d[3 * o], dst3 + 3 * i, sizeof(double) * 3);
+      t[o++] = dst_times[i];
+    }
+  }
+  CU(cudaSetDevice(ctx->device));
+  return deform_solve(ctx, node_pos3, node_times, n_nodes, s.data(), d.data(), t.data(), m, last_deform_time, nodes16, rt12,
+                      cons_nodes4, cons_weights4, out);
 }
 
 // Makes the main stream wait for the side stream's staged frame (a no-op without a pending frame): after this call every

@@ -250,6 +250,7 @@ struct EfContext {
   void* pin_small;   // results read-back
   void* dev_small;   // upload area for per-call parameters
   void* map_host;    // host-side bookkeeping of the surfel buffers (ef_map.cu)
+  void* deform;      // workspace of the deformation-graph solve (ef_deform.cu), allocated by its first call
 };
 
 // launch bookkeeping

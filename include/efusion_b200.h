@@ -115,6 +115,32 @@ typedef struct {
 } EfLoopResult;
 int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* src3, double* dst3, int32_t* times, int32_t max_constraints,
                          int32_t* n_out);
+/* Embedded-deformation solve of a local loop closure: Deformation::constrain with fernMatch = relaxGraph = false
+ * (Core/Deformation.cpp:73-207, Core/Utils/DeformationGraph.cpp). HOST inputs: the graph (node positions x3 and times, in
+ * non-decreasing time order, 5 <= n_nodes < 1024, R = I and t = 0 at the start) and the constraints (src3 = vert_w_curr at
+ * src_times, dst3 = vert_w_est at dst_times). pin != 0 adds the pin constraint (target, target, dst_time, dst_time) after each
+ * one, as the reference does while it has not deformed yet (Core/Deformation.cpp:73-86). Nodes with time <= last_deform_time
+ * are held fixed. Constraint weighting, at most 3 Gauss-Newton iterations on the normal equations (fp64, block-band
+ * Cholesky) and the hand-over run in one launch on the device. Outputs (HOST, any may be NULL except out): nodes16, 16
+ * floats per node as ef_process_frame_end takes them; rt12, the fp64 rotation (column-major) and translation of each node
+ * (12 doubles per node); cons_nodes4 / cons_weights4, the 4 nodes (ascending id) and weights
+ * of each expanded constraint. Results are deterministic: two calls on the same inputs are bit-identical. */
+typedef struct {
+  int32_t n_nodes, n_enabled, n_constraints;  /* n_constraints counts pin constraints too */
+  int32_t iterations;  /* Gauss-Newton iterations run (1..3) */
+  int32_t stop;        /* rule that ended the loop (DeformationGraph.cpp:473): 0 none (3 iterations), 1 error > lastError,
+                          2 |delta| < 1e-2, 3 error < 1e-3, 4 |errorDiff| < 1e-5 error; 5: the normal equations were not
+                          positive definite and the last delta was not applied (the reference would apply CHOLMOD's output);
+                          6: two coupled nodes lie more than 19 apart, so the band cannot hold the system and nothing was
+                          solved (the 20-node weighting window rules this out) */
+  int32_t bandwidth;   /* largest distance between two coupled enabled nodes (<= 19; 20 with stop 6) */
+  float error;         /* final squared residual norm */
+  float meanConsErr;   /* nonRelativeConstraintError after the solve */
+} EfDeformResult;
+int ef_deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int32_t n_nodes, const double* src3,
+                    const double* dst3, const int32_t* src_times, const int32_t* dst_times, int32_t n_constraints, int32_t pin,
+                    int32_t last_deform_time, float* nodes16, double* rt12, int32_t* cons_nodes4, double* cons_weights4,
+                    EfDeformResult* out);
 /* ElasticFusion::predict (Core/ElasticFusion.cpp:621-653) */
 int ef_predict(EfContext* ctx);
 
