@@ -419,6 +419,13 @@ class Context:
         n = lib().ef_debug_stage_ms(self.h_ctx, out)
         return [out[i] for i in range(n)]
 
+    def lookahead_ms(self):
+        """EF_STAGE_TIMING=1: (start, end) of the last prefetch's side-stream work, ms after the start of the frame in flight
+        when it was enqueued; None without a timed prefetch."""
+        out = (C.c_float * 2)()
+        n = lib().ef_debug_lookahead_ms(self.h_ctx, out)
+        return (out[0], out[1]) if n == 2 else None
+
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)
         _chk(lib().ef_map_upload(self.h_ctx, _p(s), len(s)))

@@ -338,6 +338,9 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
     ctx->stage_n = 0;
     if (ctx->stage_timing)
       for (int i = 0; i < 16; ++i) cudaEventCreate(&ctx->stage_ev[i]);
+    // the look-ahead's side stream starts after the frame's coarse-level cluster (default) or, EF_LA_AFTER_TRACK=0, at frame start
+    e = getenv("EF_LA_AFTER_TRACK");
+    ctx->la_after_track = !(e && e[0] == '0');
   }
   ctx->tick = 1;
   for (int k = 0; k < 16; ++k) ctx->T_wc[k] = (k % 5 == 0) ? 1.0 : 0.0;
@@ -418,6 +421,9 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
       if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.spare_free, cudaEventDisableTiming);
       if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.h2d_done, cudaEventDisableTiming);
       if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.image_ready, cudaEventDisableTiming);
+      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.track_started, cudaEventDisableTiming);
+      if (e == cudaSuccess && ctx->stage_timing) e = cudaEventCreate(&la.timing[0]);
+      if (e == cudaSuccess && ctx->stage_timing) e = cudaEventCreate(&la.timing[1]);
       if (e == cudaSuccess) e = cudaMallocHost((void**)&la.pin_rgb, n * 3);
       if (e == cudaSuccess) e = cudaMallocHost((void**)&la.pin_depth, n * 2);
       if (e != cudaSuccess) rc = (int)e;
@@ -459,6 +465,9 @@ extern "C" int ef_destroy(EfContext* ctx) {
   if (ctx->la.spare_free) cudaEventDestroy(ctx->la.spare_free);
   if (ctx->la.h2d_done) cudaEventDestroy(ctx->la.h2d_done);
   if (ctx->la.image_ready) cudaEventDestroy(ctx->la.image_ready);
+  if (ctx->la.track_started) cudaEventDestroy(ctx->la.track_started);
+  for (cudaEvent_t ev : ctx->la.timing)
+    if (ev) cudaEventDestroy(ev);
   if (ctx->la.pin_rgb) cudaFreeHost(ctx->la.pin_rgb);
   if (ctx->la.pin_depth) cudaFreeHost(ctx->la.pin_depth);
   map_free_host(ctx);
@@ -1012,6 +1021,9 @@ static int prefetch_common(EfContext* ctx, const uint8_t* rgb, const uint16_t* d
   int rc = 0;
   cudaError_t e = cudaStreamWaitEvent(la.stream, la.spare_free, 0);
   if (e == cudaSuccess) e = cudaStreamWaitEvent(la.stream, la.image_ready, 0);  // previous frame's intensity pyramid (SO(3) input)
+  if (e == cudaSuccess && la.track_marked) e = cudaStreamWaitEvent(la.stream, la.track_started, 0);
+  la.track_marked = false;
+  if (e == cudaSuccess && ctx->stage_timing) e = cudaEventRecord(la.timing[0], la.stream);
   if (e == cudaSuccess && from_host) {
     e = cudaMemcpyAsync(ctx->tex.rgb, rgb, n * 3, cudaMemcpyHostToDevice, la.stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->tex.depth_raw, depth, n * 2, cudaMemcpyHostToDevice, la.stream);
@@ -1023,6 +1035,7 @@ static int prefetch_common(EfContext* ctx, const uint8_t* rgb, const uint16_t* d
   if (!rc) rc = frame_input_side(ctx, rgb, depth);
   if (!rc) {
     e = cudaEventRecord(la.ready, la.stream);
+    if (e == cudaSuccess && ctx->stage_timing) e = cudaEventRecord(la.timing[1], la.stream);
     if (e != cudaSuccess) rc = (int)e;
   }
   ctx->stream = main_stream;
@@ -1307,6 +1320,15 @@ extern "C" int ef_debug_stage_ms(EfContext* ctx, float* out) {
     prev = i;
   }
   return 12;
+}
+// EF_STAGE_TIMING=1: milliseconds from the start of the frame in flight during the last prefetch (stage event 0) to the start of
+// the side stream's work (once its waits are met) and to its end; returns 2, or 0 without a timed prefetch.
+extern "C" int ef_debug_lookahead_ms(EfContext* ctx, float* out2) {
+  if (!ctx || !out2 || !ctx->stage_timing || !(ctx->stage_n & 1)) return 0;
+  if (cudaStreamSynchronize(ctx->la.stream) != cudaSuccess) return 0;
+  for (int i = 0; i < 2; ++i)
+    if (cudaEventElapsedTime(&out2[i], ctx->stage_ev[0], ctx->la.timing[i]) != cudaSuccess) return 0;
+  return 2;
 }
 extern "C" void* ef_debug_gn(EfContext* ctx, int which) { return ctx ? (void*)ctx->odom[which].gn : nullptr; }
 extern "C" int ef_debug_gn_size() { return (int)sizeof(GNState); }

@@ -189,6 +189,9 @@ struct Lookahead {
   cudaEvent_t spare_free;  // main stream: every reader of the spare set precedes this point
   cudaEvent_t h2d_done;    // side stream: the pinned staging buffers may be rewritten
   cudaEvent_t image_ready; // whichever stream built the newest intensity pyramid (the next frame's SO(3) loop reads it)
+  cudaEvent_t track_started;  // main stream: the frame's coarse-level cluster (or k_gn_begin) has been enqueued before this
+  bool track_marked;          // track_started was recorded by the frame in flight and the next prefetch has not waited on it
+  cudaEvent_t timing[2];   // EF_STAGE_TIMING=1: start (after its waits) and end of the side stream's work of the last prefetch
   bool pending;            // a prefetched frame is waiting to be consumed
   uint8_t *rgb, *rgba;
   uint16_t *depth_raw, *depth_filtered;
@@ -225,6 +228,7 @@ struct EfContext {
   int gn_cluster;         // CTAs of the cluster that runs the coarse-level Gauss-Newton iterations (0: two-kernel path everywhere)
   bool so3_cluster;       // the SO(3) pre-alignment loop in one cluster launch (k_so3_cluster); EF_SO3_CLUSTER=0: k_so3_begin + 10 x k_so3_step
   int gn_cluster_levels;  // pyramid levels, from the coarsest, whose iterations run in that cluster
+  bool la_after_track;    // the look-ahead's side stream starts after the frame's coarse-level cluster (EF_LA_AFTER_TRACK=0: at frame start)
   bool plain_next;     // the next ef_launch omits the programmatic-serialisation attribute (EF_PLAIN_NEXT)
   bool maps_dirty[2];  // a kernel that writes tracker w's pyramids may still be in flight ahead of the next stage launch
 

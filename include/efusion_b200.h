@@ -309,6 +309,9 @@ int ef_launch_count(EfContext* ctx, int64_t* n);
  * [1] upload + RGBA + bilateral/metric, [2] live pyramids + SO(3), [3] model pyramids, [4] sobel + candidates, [5] Gauss-Newton
  * loop, [6] finish, [7] index map, [8] fuse, [9] index map, [10] clean, [11] predict. Returns the number of slots (0 if off). */
 int ef_debug_stage_ms(EfContext* ctx, float* out16);
+/* EF_STAGE_TIMING=1: milliseconds from the start of the frame in flight during the last ef_prefetch_frame* call to the start
+ * of the side stream's work (once it may begin) and to its end, out[2]. Returns 2, or 0 without a timed prefetch. */
+int ef_debug_lookahead_ms(EfContext* ctx, float* out2);
 
 #ifdef __cplusplus
 }
