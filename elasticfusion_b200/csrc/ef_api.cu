@@ -194,6 +194,8 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   CU(cudaMemsetAsync(od.vmaps_tmp, 0, 4 * n0 * sizeof(float), ctx->stream));
   CU(A->alloc(&od.gn, 1));
   od.cand_base = reinterpret_cast<const int*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, cand_base));
+  od.intr0 = reinterpret_cast<const float*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, fx));
+  od.K_levels = reinterpret_cast<const double*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, Kd));
   CU(A->alloc(&od.so3s, 1));
   // one slot per CTA of k_so3_step, whose grid red_blocks() caps at MAX_RED_BLOCKS (254 CTAs at 1920x1080 on an H100)
   CU(A->alloc(&od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE));

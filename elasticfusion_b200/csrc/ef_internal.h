@@ -52,7 +52,7 @@ struct GNState {
   int flat_n;                   // total pixels over the three levels
   float rgbErrBuf[2];           // rgbError of the previous / current iteration (double-buffered across CTAs)
   float weighting;  // velocity weighting for fusion (ElasticFusion.cpp:369-383)
-  long long dbg[32];  // phase timestamps (clock64) when built with -DEF_PROFILE_PHASES
+  long long dbg[40];  // phase timestamps (%globaltimer) of levels 0 and 1 when built with -DEF_PROFILE_PHASES
 };
 
 // State of the SO(3) pre-alignment loop (RGBDOdometry.cpp:305-368). The loop depends only on the two intensity pyramids
@@ -97,6 +97,8 @@ struct OdomDev {
   // compacted once per frame; {pixel index, nextDepth bits, dIdx | dIdy << 16, nextImage}
   int4* cand;
   const int* cand_base;   // = gn->cand_base (device address): bounds of each level's candidates; like `cand`, final before the loop starts
+  const float* intr0;     // = &gn->fx (device address): level-0 {fx, fy, cx, cy}, written once at context creation
+  const double* K_levels; // = gn->Kd (device address): K of each level, then K^-1 of each level (gn->Kinvd); written once as well
   int4* terms;            // per candidate and iteration: {zero_x | zero_y << 16 (or -1), diff bits, dIdx | dIdy << 16, lastDepth[zero] bits}
   int level_start[NUM_PYRS + 1];  // flat pixel offset of each level
 

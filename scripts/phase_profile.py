@@ -1,34 +1,51 @@
-"""Phase timestamps (%globaltimer) of k_iter1 / k_iter2 at level 0. Needs an instrumented build of the library:
-   EF_OUT=build/libefusion_prof.so ./build.sh -DEF_PROFILE_PHASES ; EF_LIB=build/libefusion_prof.so python scripts/phase_profile.py"""
-import sys, ctypes as C, numpy as np
-import os
+"""Phase timestamps (%globaltimer) of the last k_iter1 / k_iter2 iteration of pyramid levels 0 and 1, median over frames.
+Needs an instrumented build of the library:
+   EF_OUT=build/libefusion_prof.so ./build.sh -DEF_PROFILE_PHASES ; EF_LIB=build/libefusion_prof.so python scripts/phase_profile.py [frames]"""
+import sys, os, ctypes as C, numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from elasticfusion_b200 import synth, capi
+
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 40
+SKIP = 5  # first frames: module loading, map still growing from empty
 K = synth.K_DEFAULT
-frames = list(synth.sequence(6, K, seed=42, noise=True))
+frames = list(synth.sequence(n, K, seed=42, noise=True))
 BIG = 2147483647 // 2
 ctx = capi.Context(capi.default_config(K.width, K.height, K.fx, K.fy, K.cx, K.cy, capacity=1000000, time_delta=BIG))
-for i, (rgb, d, _) in enumerate(frames):
-    ctx.process_frame(rgb, d, i)
-# GNState layout: find dbg by scanning for it via offset: use a helper export? read whole struct
-import ctypes
 lib = capi.lib()
-# read the raw GNState: ef_buffer has no id for it; use cudart directly
-cudart = C.CDLL('libcudart.so')
-ptr = C.c_void_p(); n = C.c_size_t()
-# trick: the gn pointer is not exposed; add a debug export
+cudart = C.CDLL("libcudart.so")
 lib.ef_debug_gn.restype = C.c_void_p
 gnp = lib.ef_debug_gn(ctx.h_ctx, 0)
 sz = lib.ef_debug_gn_size()
-buf = (C.c_char * sz)()
-cudart.cudaMemcpy(buf, C.c_void_p(gnp), C.c_size_t(sz), 2)
 off = lib.ef_debug_dbg_offset()
-dbg = np.frombuffer(buf, dtype=np.int64, count=32, offset=off)
-d = dbg.astype(np.int64)
-print("globaltimer ns, last level-0 iteration (block 0 / last block stamps)")
-print("k_iter1: start->cand done %d, icp loop %d, block reduce %d   [k1 total %d]" % (d[1]-d[0], d[2]-d[1], d[3]-d[2], d[3]-d[0]))
-print("k1.end(block0) -> k2.start(block0): %d" % (d[8]-d[3]))
-print("k_iter2 block0: stats %d, rgb+presum %d" % (d[9]-d[8], d[10]-d[9]))
-print("k2 block0 done -> last block has ticket: %d" % (d[11]-d[10]))
-print("k_iter2 last block: final sums %d, stage+lastA %d, ldlt %d, rodrigues %d, rest %d" % (d[12]-d[11], d[13]-d[12], d[14]-d[13], d[15]-d[14], d[16]-d[15]))
-print("k1.start -> k2.end: %d" % (d[16]-d[0]))
+buf = (C.c_char * sz)()
+stamps = []
+for i, (rgb, d, _) in enumerate(frames):
+    ctx.process_frame(rgb, d, i)
+    if cudart.cudaDeviceSynchronize() != 0 or cudart.cudaMemcpy(buf, C.c_void_p(gnp), C.c_size_t(sz), 2) != 0:
+        raise RuntimeError("reading the GN state failed")
+    if i >= SKIP:
+        stamps.append(np.frombuffer(buf, dtype=np.int64, count=40, offset=off).copy())
+S = np.array(stamps)
+
+# (name, first slot, last slot) of each phase; slots of level L are 20 * L + s
+PHASES = [
+    ("k_iter1: photometric correspondences", 0, 1),
+    ("k_iter1: dense geometric rows", 1, 2),
+    ("k_iter1: block reduce + partial", 2, 3),
+    ("k_iter1 end -> k_iter2 start (block 0)", 3, 8),
+    ("k_iter2: statistics", 8, 9),
+    ("k_iter2: photometric rows + presum", 9, 10),
+    ("k_iter2: block 0 done -> last ticket", 10, 11),
+    ("tail: final sums", 11, 12),
+    ("tail: unpack + lastA/lastb", 12, 13),
+    ("tail: LDL^T solve", 13, 14),
+    ("tail: Rodrigues", 14, 15),
+    ("tail: pose, warp and stores", 15, 16),
+]
+print(f"globaltimer ns, median over {len(S)} frames (the last iteration of each level in each frame)")
+print(f"{'phase':42s} {'level 0':>8s} {'level 1':>8s}")
+for name, a, b in PHASES:
+    print(f"{name:42s} " + " ".join(f"{np.median(S[:, 20 * L + b] - S[:, 20 * L + a]):8.0f}" for L in (0, 1)))
+for name, a, b in [("k_iter2 statistics (block 0)", 8, 9), ("post-ticket tail", 11, 16), ("k_iter1 start -> tail end", 0, 16)]:
+    print(f"{name:42s} " + " ".join(f"{np.median(S[:, 20 * L + b] - S[:, 20 * L + a]):8.0f}" for L in (0, 1)))
+ctx.close()
