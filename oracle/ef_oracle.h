@@ -181,6 +181,8 @@ void efo_fusion_process_frame_deform(EfoFusion* f, const uint8_t* rgb, const uin
 void efo_fusion_destroy(EfoFusion* f);
 void efo_fusion_process_frame(EfoFusion* f, const uint8_t* rgb, const uint16_t* depth, int64_t timestamp,
                               float weight_multiplier, const double* in_T_wc16);
+/* test setup: the model becomes surfels12[0 .. min(n, capacity)) and predict() re-renders the model view (tick unchanged) */
+void efo_fusion_set_map(EfoFusion* f, const float* surfels12, int n);
 void efo_fusion_pose(const EfoFusion* f, double* T_wc16);
 int efo_fusion_count(const EfoFusion* f);
 int efo_fusion_tick(const EfoFusion* f);

@@ -468,6 +468,11 @@ class Fusion:
         lib().efo_fusion_process_frame_deform(self.hnd, _p(rgb), _p(depth), C.c_int64(timestamp), _f(weight_multiplier), _p(T), _p(To),
                                               _p(nd), 0 if nd is None else len(nd), int(fern_accepted))
 
+    def set_map(self, surfels):
+        """Replaces the model by `surfels` ((n, 12) float32, cut to the capacity) and re-renders the model view (predict())."""
+        s = np.ascontiguousarray(surfels, np.float32).reshape(-1, 12)
+        lib().efo_fusion_set_map(self.hnd, _p(s), len(s))
+
     def set_loop_closure(self, enabled=True, count_thresh=35000, err_thresh=5e-05, cov_thresh=1e-05):
         lib().efo_fusion_set_loop_closure(self.hnd, int(enabled), int(count_thresh), _f(err_thresh), _f(cov_thresh))
 

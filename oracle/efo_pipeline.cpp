@@ -320,6 +320,14 @@ extern "C" void efo_fusion_process_frame_deform(EfoFusion* f, const uint8_t* rgb
   f->tick++;
 }
 
+// Replaces the model by n surfels (at most `capacity`) and re-renders the model view with predict(), as a caller that loads a map
+// after the first frame would; the frame inputs predict() fills in from (filtered depth, colour) stay those of the last frame.
+extern "C" void efo_fusion_set_map(EfoFusion* f, const float* surfels12, int n) {
+  f->count = std::max(0, std::min(n, f->cfg.capacity));
+  if (f->count > 0) memcpy(f->map.data(), surfels12, sizeof(float) * 12 * (size_t)f->count);
+  predict(f);
+}
+
 extern "C" void efo_fusion_set_tracker(EfoFusion* f, const EfoTrackerBackend* b) {
   f->has_ext = b != nullptr;
   if (b) f->ext = *b;
