@@ -222,13 +222,9 @@ struct EfContext {
   cudaEvent_t stage_ev[16];
   int stage_n;
   bool pdl;  // programmatic dependent launch on every kernel (default on; EF_NO_PDL=1 disables)
-  bool it1_prefetch;   // k_iter1 loads its first round of live-map pixels before griddepcontrol.wait (EF_IT1_PREFETCH=0 disables)
-  int it2_max_blocks;  // cap on k_iter2's grid (EF_IT2_MAXBLOCKS; default MAX_RGB_BLOCKS)
-  bool vis_pending;       // the first pass of a frame has filled the visible list and the second has not consumed it yet
+  bool vis_pending;      // the first pass of a frame has filled the visible list and the second has not consumed it yet
   bool visible_list;      // second index-map pass of a frame visits only the surfels the first one rasterised; EF_VISIBLE_LIST=0 disables
-  bool fused_model_side;  // model pyramids of a frame in 3 launches (k_model_level0 / _down) instead of 6; EF_FUSED_MODEL=0 disables
-  int gn_cluster;         // CTAs of the cluster that runs the coarse-level Gauss-Newton iterations (0: two-kernel path everywhere)
-  bool so3_cluster;       // the SO(3) pre-alignment loop in one cluster launch (k_so3_cluster); EF_SO3_CLUSTER=0: k_so3_begin + 10 x k_so3_step
+  int gn_cluster;         // CTAs of the clusters that run the SO(3) loop and the coarse-level Gauss-Newton iterations (0: plain launches everywhere)
   int gn_cluster_levels;  // pyramid levels, from the coarsest, whose iterations run in that cluster
   bool la_after_track;    // the look-ahead's side stream starts after the frame's coarse-level cluster (EF_LA_AFTER_TRACK=0: at frame start)
   bool plain_next;     // the next ef_launch omits the programmatic-serialisation attribute (EF_PLAIN_NEXT)

@@ -32,13 +32,11 @@ import bench  # noqa: E402  (make_frames, workload, gpu_info; nothing runs at im
 CONFIGS = {
     "default": {},
     "at_frame_start": {"EF_LA_AFTER_TRACK": "0"},
-    "at_frame_start+so3_cluster=0": {"EF_LA_AFTER_TRACK": "0", "EF_SO3_CLUSTER": "0"},
     "at_frame_start+gn_cluster=8": {"EF_LA_AFTER_TRACK": "0", "EF_GN_CLUSTER": "8"},
     "at_frame_start+gn_cluster=0": {"EF_LA_AFTER_TRACK": "0", "EF_GN_CLUSTER": "0"},
-    "so3_cluster=0": {"EF_SO3_CLUSTER": "0"},
     "gn_cluster=0": {"EF_GN_CLUSTER": "0"},
 }
-SWITCHES = ("EF_LA_AFTER_TRACK", "EF_SO3_CLUSTER", "EF_GN_CLUSTER", "EF_STAGE_TIMING")
+SWITCHES = ("EF_LA_AFTER_TRACK", "EF_GN_CLUSTER", "EF_STAGE_TIMING")
 
 
 def make_ctx(capi, cfg, stream, env):

@@ -554,7 +554,7 @@ def test_cluster_and_two_kernel_gauss_newton_agree(monkeypatch):
     vtx, nrm, img = f.buffer("fill_vertex"), f.buffer("fill_normal"), f.buffer("fill_image")
 
     def run(env):
-        for k in ("EF_GN_CLUSTER", "EF_GN_CLUSTER_LEVELS", "EF_SO3_CLUSTER"):
+        for k in ("EF_GN_CLUSTER", "EF_GN_CLUSTER_LEVELS"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -578,7 +578,7 @@ def test_cluster_and_two_kernel_gauss_newton_agree(monkeypatch):
         finally:
             ctx.close()
 
-    ref = run({"EF_GN_CLUSTER": "0", "EF_SO3_CLUSTER": "0"})  # launches only: k_so3_step, k_iter1, k_iter2
+    ref = run({"EF_GN_CLUSTER": "0"})  # launches only: k_so3_step, k_iter1, k_iter2
     for env in ({"EF_GN_CLUSTER": "16", "EF_GN_CLUSTER_LEVELS": "3"}, {}, {"EF_GN_CLUSTER": "8", "EF_GN_CLUSTER_LEVELS": "2"},
                 {"EF_GN_CLUSTER": "16", "EF_GN_CLUSTER_LEVELS": "2"}):
         got = run(env)
