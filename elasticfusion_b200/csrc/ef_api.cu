@@ -15,90 +15,6 @@
 
 using namespace ef;
 
-// ---- kernels' host entry points (ef_track.cu, ef_preprocess.cu, ef_map.cu) --------------------------------------
-namespace ef {
-int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff);
-int odom_init_icp_pred(EfContext* ctx, int which, const float* vtx4, const float* nrm4);
-int odom_init_icp_model(EfContext* ctx, int which, const float* vtx4, const float* nrm4, bool with_global = true);
-int odom_populate(EfContext* ctx, int which, const uint8_t* rgba, float** destDepths, uint8_t** destImages, bool with_depth,
-                  bool with_image = true);
-int odom_cluster_size(int want);
-int odom_track_async(EfContext* ctx, int which, bool rgbOnly, float icpWeight, bool pyramid, bool fastOdom, bool so3);
-int odom_finish_async(EfContext* ctx, int which, float weightMultiplier, bool have_track);
-int odom_set_pose_async(EfContext* ctx, int which, const double* T_dev);
-int launch_se3_step_raw(EfContext* ctx, int which, int level, bool do_icp, bool do_rgb, float sigma);
-int launch_rgb_residual_raw(EfContext* ctx, int which, int level);
-int launch_icp_dense_only(EfContext* ctx, int which, int level);
-int launch_so3_raw(EfContext* ctx, int which);
-int launch_sobel(EfContext* ctx, int which);
-int odom_so3_async(EfContext* ctx, int which);
-int preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric, float* metric_filtered);
-int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba);
-
-int map_initialise_async(EfContext* ctx);
-int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
-int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, int time_delta, int vis_mode = 0);
-int map_fuse_async(EfContext* ctx, int time_or_neg, float max_depth, float weighting_or_neg);
-int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0, bool is_fern = false);
-int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);
-int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
-int map_loop_reset_async(EfContext* ctx);
-int odom_copy_pose_async(EfContext* ctx, int dst, int src);
-int map_resize_to_host(EfContext* ctx, const void* src_dev, int elem, int factor, void* host_out);
-int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode,
-                      bool use_device_tick);
-int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
-int map_dense_enough_async(EfContext* ctx);
-int map_tick_increment_async(EfContext* ctx);
-int map_select_model_inputs(EfContext* ctx, const float** vtx, const float** nrm, const uint8_t** img);
-void map_free_host(EfContext* ctx);
-
-int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
-                 const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
-                 int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out);
-void deform_free(EfContext* ctx);
-}  // namespace ef
-
-#define CU(x)                                  \
-  do {                                         \
-    cudaError_t e__ = (x);                     \
-    if (e__ != cudaSuccess) return (int)e__;   \
-  } while (0)
-#define RC(x)              \
-  do {                     \
-    int rc__ = (x);        \
-    if (rc__) return rc__; \
-  } while (0)
-
-namespace {
-
-struct Arena {
-  std::vector<void*> blocks;
-  template <typename T>
-  cudaError_t alloc(T** p, size_t n) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, n * sizeof(T) + 256);
-    if (e != cudaSuccess) return e;
-    blocks.push_back(q);
-    *p = (T*)q;
-    return cudaSuccess;
-  }
-};
-
-
-struct CtxExtra {
-  Arena arena;
-  std::vector<EfSolveTrace> trace_host;
-};
-
-}  // namespace
-
-struct EfContextFull : EfContext {
-  CtxExtra extra;
-};
-
-static Arena* arena(EfContext* ctx) { return &static_cast<EfContextFull*>(ctx)->extra.arena; }
-
 extern "C" void ef_default_config(EfConfig* c, int width, int height, float fx, float fy, float cx, float cy) {
   memset(c, 0, sizeof(*c));
   c->width = width;
@@ -138,7 +54,6 @@ extern "C" const char* ef_error_string(int code) {
 }
 
 static int alloc_odom(EfContext* ctx, OdomDev& od) {
-  Arena* A = arena(ctx);
   const EfConfig& c = ctx->cfg;
   memset(&od, 0, sizeof(od));
   od.width = c.width;
@@ -157,60 +72,38 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
     od.rows[i] = c.height >> i;
     od.cols[i] = c.width >> i;
     const size_t n = (size_t)od.rows[i] * od.cols[i];
-    CU(A->alloc(&od.depth_tmp[i], n));
-    CU(A->alloc(&od.vmap_g_prev[i], 3 * n));
-    CU(A->alloc(&od.nmap_g_prev[i], 3 * n));
-    CU(A->alloc(&od.vmap_c_prev[i], 3 * n));
-    CU(A->alloc(&od.nmap_c_prev[i], 3 * n));
-    CU(A->alloc(&od.vmap_curr[i], 3 * n));
-    CU(A->alloc(&od.nmap_curr[i], 3 * n));
-    CU(A->alloc(&od.lastDepth[i], n));
-    CU(A->alloc(&od.nextDepth[i], n));
-    CU(A->alloc(&od.lastImage[i], n));
-    CU(A->alloc(&od.nextImage[i], n));
-    CU(A->alloc(&od.lastNextImage[i], n));
-    CU(A->alloc(&od.dIdx[i], n));
-    CU(A->alloc(&od.dIdy[i], n));
-    CU(A->alloc(&od.corres[i], n));
     // the reference's cudaMalloc'd maps start uninitialised; NaN / zero fill keeps every first read defined
-    CU(cudaMemsetAsync(od.vmap_g_prev[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.nmap_g_prev[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.vmap_c_prev[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.nmap_c_prev[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.vmap_curr[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.nmap_curr[i], 0xff, 3 * n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.lastDepth[i], 0xff, n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.nextDepth[i], 0xff, n * sizeof(float), ctx->stream));
-    CU(cudaMemsetAsync(od.lastImage[i], 0, n, ctx->stream));
-    CU(cudaMemsetAsync(od.nextImage[i], 0, n, ctx->stream));
-    CU(cudaMemsetAsync(od.lastNextImage[i], 0, n, ctx->stream));
-    CU(cudaMemsetAsync(od.dIdx[i], 0, n * 2, ctx->stream));
-    CU(cudaMemsetAsync(od.dIdy[i], 0, n * 2, ctx->stream));
-    CU(cudaMemsetAsync(od.corres[i], 0, n * sizeof(DataTerm), ctx->stream));
-    CU(cudaMemsetAsync(od.depth_tmp[i], 0, n * 2, ctx->stream));
+    CU(ctx_alloc(ctx, &od.depth_tmp[i], n, 0));
+    CU(ctx_alloc(ctx, &od.vmap_g_prev[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.nmap_g_prev[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.vmap_c_prev[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.nmap_c_prev[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.vmap_curr[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.nmap_curr[i], 3 * n, 0xff));
+    CU(ctx_alloc(ctx, &od.lastDepth[i], n, 0xff));
+    CU(ctx_alloc(ctx, &od.nextDepth[i], n, 0xff));
+    CU(ctx_alloc(ctx, &od.lastImage[i], n, 0));
+    CU(ctx_alloc(ctx, &od.nextImage[i], n, 0));
+    CU(ctx_alloc(ctx, &od.lastNextImage[i], n, 0));
+    CU(ctx_alloc(ctx, &od.dIdx[i], n, 0));
+    CU(ctx_alloc(ctx, &od.dIdy[i], n, 0));
+    CU(ctx_alloc(ctx, &od.corres[i], n, 0));
   }
   const size_t n0 = (size_t)c.width * c.height;
-  CU(A->alloc(&od.vmaps_tmp, 4 * n0));
-  CU(cudaMemsetAsync(od.vmaps_tmp, 0, 4 * n0 * sizeof(float), ctx->stream));
-  CU(A->alloc(&od.gn, 1));
+  CU(ctx_alloc(ctx, &od.vmaps_tmp, 4 * n0, 0));
+  CU(ctx_alloc(ctx, &od.gn, 1));
   od.cand_base = reinterpret_cast<const int*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, cand_base));
   od.intr0 = reinterpret_cast<const float*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, fx));
   od.K_levels = reinterpret_cast<const double*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, Kd));
-  CU(A->alloc(&od.so3s, 1));
+  CU(ctx_alloc(ctx, &od.so3s, 1, 0));
   // one slot per CTA of k_so3_step, whose grid red_blocks() caps at MAX_RED_BLOCKS (254 CTAs at 1920x1080 on an H100)
-  CU(A->alloc(&od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE));
-  CU(A->alloc(&od.so3_counter, 4));
-  CU(cudaMemsetAsync(od.so3s, 0, sizeof(So3State), ctx->stream));
-  CU(cudaMemsetAsync(od.so3_counter, 0, 16, ctx->stream));
-  CU(A->alloc(&od.partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE));
-  CU(A->alloc(&od.partials_rgb, (size_t)MAX_RGB_BLOCKS * 32));
-  CU(A->alloc(&od.partials2, (size_t)MAX_RGB_BLOCKS * 32));
-  // (the reductions read whole 32-float rows of these; the kernels write the 29 / 11 terms of a system, so the padding lanes
-  // are defined once here)
-  CU(cudaMemsetAsync(od.so3_partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream));
-  CU(cudaMemsetAsync(od.partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream));
-  CU(cudaMemsetAsync(od.partials_rgb, 0, (size_t)MAX_RGB_BLOCKS * 32 * sizeof(float), ctx->stream));
-  CU(cudaMemsetAsync(od.partials2, 0, (size_t)MAX_RGB_BLOCKS * 32 * sizeof(double), ctx->stream));
+  // (the reductions read whole 32-float rows of the partials; the kernels write the 29 / 11 terms of a system, so the padding
+  // lanes are defined once here)
+  CU(ctx_alloc(ctx, &od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
+  CU(ctx_alloc(ctx, &od.so3_counter, 4, 0));
+  CU(ctx_alloc(ctx, &od.partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
+  CU(ctx_alloc(ctx, &od.partials_rgb, (size_t)MAX_RGB_BLOCKS * 32, 0));
+  CU(ctx_alloc(ctx, &od.partials2, (size_t)MAX_RGB_BLOCKS * 32, 0));
   {
     size_t flat = 0;
     for (int i = 0; i < NUM_PYRS; ++i) {
@@ -218,16 +111,12 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
       flat += (size_t)od.rows[i] * od.cols[i];
     }
     od.level_start[NUM_PYRS] = (int)flat;
-    CU(A->alloc(&od.cand, flat));
-    CU(A->alloc(&od.terms, flat));
-    CU(cudaMemsetAsync(od.cand, 0, flat * sizeof(int4), ctx->stream));
-    CU(cudaMemsetAsync(od.terms, 0, flat * sizeof(int4), ctx->stream));
+    CU(ctx_alloc(ctx, &od.cand, flat, 0));
+    CU(ctx_alloc(ctx, &od.terms, flat, 0));
   }
-  CU(A->alloc(&od.partials_i, (size_t)MAX_RED_BLOCKS * 2));
-  CU(A->alloc(&od.counter, 4));
-  CU(A->alloc(&od.trace, MAX_TRACE));
-  CU(cudaMemsetAsync(od.counter, 0, 16, ctx->stream));
-  CU(cudaMemsetAsync(od.trace, 0, sizeof(EfSolveTrace) * MAX_TRACE, ctx->stream));
+  CU(ctx_alloc(ctx, &od.partials_i, (size_t)MAX_RED_BLOCKS * 2));
+  CU(ctx_alloc(ctx, &od.counter, 4, 0));
+  CU(ctx_alloc(ctx, &od.trace, MAX_TRACE, 0));
   GNState g;
   memset(&g, 0, sizeof(g));
   for (int k = 0; k < 16; ++k) g.T_wc[k] = (k % 5 == 0) ? 1.0 : 0.0;
@@ -255,27 +144,77 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   return 0;
 }
 
-namespace ef {
-int alloc_map(EfContext* ctx);  // ef_map.cu
+// every buffer, stream and event of a context, in order; returns on the first error (ef_destroy frees whatever was made)
+static int create_buffers(EfContext* ctx) {
+  RC(alloc_odom(ctx, ctx->odom[0]));
+  RC(alloc_odom(ctx, ctx->odom[1]));
+  const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
+  Textures& t = ctx->tex;
+  memset(&t, 0, sizeof(t));
+  CU(ctx_alloc(ctx, &t.rgb, n * 3, 0));
+  CU(ctx_alloc(ctx, &t.rgba, n * 4, 0));
+  CU(ctx_alloc(ctx, &t.depth_raw, n, 0));
+  CU(ctx_alloc(ctx, &t.depth_filtered, n, 0));
+  CU(ctx_alloc(ctx, &t.depth_metric, n, 0));
+  CU(ctx_alloc(ctx, &t.depth_metric_filtered, n, 0));
+  CU(ctx_alloc(ctx, &t.index, n, 0));
+  CU(ctx_alloc(ctx, &t.vert_conf, n, 0));
+  CU(ctx_alloc(ctx, &t.color_time, n, 0));
+  CU(ctx_alloc(ctx, &t.norm_rad, n, 0));
+  CU(ctx_alloc(ctx, &t.image, n, 0));
+  CU(ctx_alloc(ctx, &t.old_image, n, 0));
+  CU(ctx_alloc(ctx, &t.fill_image, n, 0));
+  CU(ctx_alloc(ctx, &t.vertex, n, 0));
+  CU(ctx_alloc(ctx, &t.normal, n, 0));
+  CU(ctx_alloc(ctx, &t.old_vertex, n, 0));
+  CU(ctx_alloc(ctx, &t.old_normal, n, 0));
+  CU(ctx_alloc(ctx, &t.fill_vertex, n, 0));
+  CU(ctx_alloc(ctx, &t.fill_normal, n, 0));
+  CU(ctx_alloc(ctx, &t.time, n, 0));
+  CU(ctx_alloc(ctx, &t.old_time, n, 0));
+  CU(ctx_alloc(ctx, &t.synth_depth, n, 0));
+  // spare input-side set + side stream of the frame look-ahead
+  Lookahead& la = ctx->la;
+  memset(&la, 0, sizeof(la));
+  CU(ctx_alloc(ctx, &la.rgb, n * 3, 0));
+  CU(ctx_alloc(ctx, &la.rgba, n * 4, 0));
+  CU(ctx_alloc(ctx, &la.depth_raw, n, 0));
+  CU(ctx_alloc(ctx, &la.depth_filtered, n, 0));
+  CU(ctx_alloc(ctx, &la.depth_metric, n, 0));
+  CU(ctx_alloc(ctx, &la.depth_metric_filtered, n, 0));
+  for (int i = 0; i < NUM_PYRS; ++i) {
+    const size_t ni = (size_t)ctx->odom[0].rows[i] * ctx->odom[0].cols[i];
+    CU(ctx_alloc(ctx, &la.depth_tmp[i], ni, 0));
+    CU(ctx_alloc(ctx, &la.vmap_curr[i], 3 * ni, 0xff));
+    CU(ctx_alloc(ctx, &la.nmap_curr[i], 3 * ni, 0xff));
+    CU(ctx_alloc(ctx, &la.image[i], ni, 0));
+  }
+  CU(ctx_alloc(ctx, &la.so3s, 1, 0));
+  CU(ctx_alloc(ctx, &la.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
+  CU(ctx_alloc(ctx, &la.so3_counter, 4, 0));
+  CU(cudaStreamCreateWithFlags(&la.stream, cudaStreamNonBlocking));
+  CU(cudaEventCreateWithFlags(&la.ready, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&la.spare_free, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&la.h2d_done, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&la.image_ready, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&la.track_started, cudaEventDisableTiming));
+  if (ctx->stage_timing) {
+    CU(cudaEventCreate(&la.timing[0]));
+    CU(cudaEventCreate(&la.timing[1]));
+  }
+  CU(cudaMallocHost((void**)&la.pin_rgb, n * 3));
+  CU(cudaMallocHost((void**)&la.pin_depth, n * 2));
+  RC(alloc_map(ctx));
+  CU(cudaMallocHost((void**)&ctx->pin_rgb, n * 3));
+  CU(cudaMallocHost((void**)&ctx->pin_depth, n * 2));
+  CU(cudaMallocHost((void**)&ctx->pin_small, sizeof(PinStaging)));
+  CU(cudaMalloc((void**)&ctx->dev_small, sizeof(DevStaging)));
+  CU(cudaEventRecord(la.spare_free, ctx->stream));
+  CU(cudaEventRecord(la.h2d_done, la.stream));
+  CU(cudaEventRecord(la.image_ready, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
 }
-namespace ef {
-template <typename T>
-cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n) {
-  return arena(ctx)->alloc(p, n);
-}
-template cudaError_t ctx_alloc<float4>(EfContext*, float4**, size_t);
-template cudaError_t ctx_alloc<float>(EfContext*, float**, size_t);
-template cudaError_t ctx_alloc<double>(EfContext*, double**, size_t);
-template cudaError_t ctx_alloc<int>(EfContext*, int**, size_t);
-template cudaError_t ctx_alloc<unsigned int>(EfContext*, unsigned int**, size_t);
-template cudaError_t ctx_alloc<unsigned long long>(EfContext*, unsigned long long**, size_t);
-template cudaError_t ctx_alloc<uint8_t>(EfContext*, uint8_t**, size_t);
-template cudaError_t ctx_alloc<uint16_t>(EfContext*, uint16_t**, size_t);
-template cudaError_t ctx_alloc<uchar4>(EfContext*, uchar4**, size_t);
-template cudaError_t ctx_alloc<MapPose>(EfContext*, MapPose**, size_t);
-template cudaError_t ctx_alloc<int4>(EfContext*, int4**, size_t);
-template cudaError_t ctx_alloc<LoopDev>(EfContext*, LoopDev**, size_t);
-}  // namespace ef
 
 extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
   if (!cfg || !out || cfg->width <= 0 || cfg->height <= 0 || cfg->capacity <= 0) return EF_EINVAL;
@@ -284,9 +223,8 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
   if (cfg->reloc) return EF_EINVAL;
   if ((cfg->width >> 2) < 8 || (cfg->height >> 2) < 8) return EF_EINVAL;
   CU(cudaSetDevice(cfg->device));
-  EfContextFull* full = new (std::nothrow) EfContextFull();
-  if (!full) return EF_ENOMEM;
-  EfContext* ctx = full;
+  EfContext* ctx = new (std::nothrow) EfContext();
+  if (!ctx) return EF_ENOMEM;
   ctx->cfg = *cfg;
   ctx->device = cfg->device;
   {
@@ -303,7 +241,7 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
       }
     }
     if (e != cudaSuccess) {  // nothing else has been allocated yet
-      delete full;
+      delete ctx;
       return (int)e;
     }
   }
@@ -349,96 +287,7 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
   ctx->host_count = 0;
   ctx->frame_open = false;
 
-  int rc = alloc_odom(ctx, ctx->odom[0]);
-  if (!rc) rc = alloc_odom(ctx, ctx->odom[1]);
-  const size_t n = (size_t)cfg->width * cfg->height;
-  Arena* A = arena(ctx);
-  Textures& t = ctx->tex;
-  memset(&t, 0, sizeof(t));
-#define TA(p, cnt)                               \
-  if (!rc) {                                     \
-    cudaError_t e_ = A->alloc(&(p), (cnt));      \
-    if (e_ != cudaSuccess) rc = (int)e_;         \
-    else cudaMemsetAsync((p), 0, (cnt) * sizeof(*(p)), ctx->stream); \
-  }
-  TA(t.rgb, n * 3);
-  TA(t.rgba, n * 4);
-  TA(t.depth_raw, n);
-  TA(t.depth_filtered, n);
-  TA(t.depth_metric, n);
-  TA(t.depth_metric_filtered, n);
-  TA(t.index, n);
-  TA(t.vert_conf, n);
-  TA(t.color_time, n);
-  TA(t.norm_rad, n);
-  TA(t.image, n);
-  TA(t.old_image, n);
-  TA(t.fill_image, n);
-  TA(t.vertex, n);
-  TA(t.normal, n);
-  TA(t.old_vertex, n);
-  TA(t.old_normal, n);
-  TA(t.fill_vertex, n);
-  TA(t.fill_normal, n);
-  TA(t.time, n);
-  TA(t.old_time, n);
-  TA(t.synth_depth, n);
-  {
-    // spare input-side set + side stream of the frame look-ahead
-    Lookahead& la = ctx->la;
-    memset(&la, 0, sizeof(la));
-    TA(la.rgb, n * 3);
-    TA(la.rgba, n * 4);
-    TA(la.depth_raw, n);
-    TA(la.depth_filtered, n);
-    TA(la.depth_metric, n);
-    TA(la.depth_metric_filtered, n);
-    for (int i = 0; i < NUM_PYRS; ++i) {
-      const size_t ni = (size_t)ctx->odom[0].rows[i] * ctx->odom[0].cols[i];
-      TA(la.depth_tmp[i], ni);
-      TA(la.vmap_curr[i], 3 * ni);
-      TA(la.nmap_curr[i], 3 * ni);
-      TA(la.image[i], ni);
-      if (!rc) {
-        cudaMemsetAsync(la.vmap_curr[i], 0xff, 3 * ni * sizeof(float), ctx->stream);
-        cudaMemsetAsync(la.nmap_curr[i], 0xff, 3 * ni * sizeof(float), ctx->stream);
-      }
-    }
-    TA(la.so3s, 1);
-    TA(la.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE);
-    TA(la.so3_counter, 4);
-    if (!rc) cudaMemsetAsync(la.so3_partials, 0, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE * sizeof(float), ctx->stream);
-    if (!rc) {
-      cudaError_t e = cudaStreamCreateWithFlags(&la.stream, cudaStreamNonBlocking);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.ready, cudaEventDisableTiming);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.spare_free, cudaEventDisableTiming);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.h2d_done, cudaEventDisableTiming);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.image_ready, cudaEventDisableTiming);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&la.track_started, cudaEventDisableTiming);
-      if (e == cudaSuccess && ctx->stage_timing) e = cudaEventCreate(&la.timing[0]);
-      if (e == cudaSuccess && ctx->stage_timing) e = cudaEventCreate(&la.timing[1]);
-      if (e == cudaSuccess) e = cudaMallocHost((void**)&la.pin_rgb, n * 3);
-      if (e == cudaSuccess) e = cudaMallocHost((void**)&la.pin_depth, n * 2);
-      if (e != cudaSuccess) rc = (int)e;
-    }
-  }
-#undef TA
-  if (!rc) rc = alloc_map(ctx);
-  if (!rc) {
-    cudaError_t e = cudaMallocHost((void**)&ctx->pin_rgb, n * 3);
-    if (e == cudaSuccess) e = cudaMallocHost((void**)&ctx->pin_depth, n * 2);
-    if (e == cudaSuccess) e = cudaMallocHost(&ctx->pin_small, 65536);
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->dev_small, 65536);
-    if (e != cudaSuccess) rc = (int)e;
-  }
-  if (!rc) {
-    cudaError_t e = cudaEventRecord(ctx->la.spare_free, ctx->stream);
-    if (e == cudaSuccess) e = cudaEventRecord(ctx->la.h2d_done, ctx->la.stream);
-    if (e == cudaSuccess) e = cudaEventRecord(ctx->la.image_ready, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) rc = (int)e;
-  }
-  if (rc) {
+  if (int rc = create_buffers(ctx)) {
     ef_destroy(ctx);
     return rc;
   }
@@ -465,13 +314,13 @@ extern "C" int ef_destroy(EfContext* ctx) {
   if (ctx->la.pin_depth) cudaFreeHost(ctx->la.pin_depth);
   map_free_host(ctx);
   deform_free(ctx);
-  for (void* p : arena(ctx)->blocks) cudaFree(p);
+  ctx->arena.release();
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
   if (ctx->pin_small) cudaFreeHost(ctx->pin_small);
   if (ctx->dev_small) cudaFree(ctx->dev_small);
   if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
-  delete static_cast<EfContextFull*>(ctx);
+  delete ctx;
   return 0;
 }
 
@@ -674,7 +523,7 @@ extern "C" int ef_icp_step_async(EfContext* ctx, int which, int level, const flo
                                  const float* tprev) {
   if (!ctx || !WHICH_OK(which) || level < 0 || level >= NUM_PYRS) return EF_EINVAL;
   if (Rcurr) {
-    float* s = (float*)ctx->pin_small;
+    float* s = ctx->pin_small->icp_inputs;
     CU(cudaStreamSynchronize(ctx->stream));  // the H2D copies of the previous call may still be reading the staging buffer
     memcpy(s, Rcurr, 36);
     memcpy(s + 9, tcurr, 12);
@@ -804,13 +653,6 @@ extern "C" int ef_set_depth_cutoff(EfContext* ctx, float v) { if (!ctx) return E
 // ---------------------------------------------------------------------------------------------------------------
 // map stage API
 // ---------------------------------------------------------------------------------------------------------------
-namespace ef {
-int map_download(EfContext* ctx, const float4* a, const float4* b, const float4* c, int n, float* out);
-int map_upload(EfContext* ctx, const float* in, int n);
-int map_upload_range(EfContext* ctx, const float* in, int first, int n);
-void map_free_host(EfContext* ctx);
-}
-
 static int read_count(EfContext* ctx, const int* dev, int* out) {
   CU(cudaMemcpyAsync(out, dev, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -847,7 +689,7 @@ extern "C" int ef_map_raycast(EfContext* ctx, const double* T, float max_depth, 
                               int32_t time_delta, int32_t mode) {
   if (!ctx || mode < 0 || mode > 2) return EF_EINVAL;
   RC(map_update_pose_async(ctx, T));
-  return map_raycast_async(ctx, max_depth, conf_threshold, time, max_time, time_delta, mode, false);
+  return map_raycast_async(ctx, max_depth, conf_threshold, time, max_time, time_delta, mode);
 }
 extern "C" int ef_map_fill_in(EfContext* ctx, int32_t pass_geom, int32_t pass_img) {
   if (!ctx) return EF_EINVAL;
@@ -895,7 +737,7 @@ extern "C" int ef_map_upload(EfContext* ctx, const float* in12, int32_t count) {
 // ---------------------------------------------------------------------------------------------------------------
 // ElasticFusion::predict, reference Core/ElasticFusion.cpp:621-653 (lost == false, lastFrameRecovery == false)
 static int predict_async(EfContext* ctx) {
-  RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick, ctx->cfg.time_delta, 0, false));
+  RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick, ctx->cfg.time_delta, 0));
   return map_fill_in_async(ctx, false, ctx->frame_to_frame_rgb);
 }
 
@@ -1009,7 +851,7 @@ extern "C" int ef_prefetch_frame(EfContext* ctx, const uint8_t* rgb, const uint1
 static int local_loop_async(EfContext* ctx) {
   Textures& t = ctx->tex;
   OdomDev& od = ctx->odom[1];
-  RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, 0, ctx->tick - ctx->cfg.time_delta, ctx->cfg.time_delta, 1, false));
+  RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, 0, ctx->tick - ctx->cfg.time_delta, ctx->cfg.time_delta, 1));
   RC(odom_copy_pose_async(ctx, 1, 0));
   RC(odom_init_icp_model(ctx, 1, (const float*)t.old_vertex, (const float*)t.old_normal, false));
   RC(odom_populate(ctx, 1, (const uint8_t*)t.old_image, od.lastDepth, od.lastImage, true));
@@ -1053,7 +895,7 @@ static int frame_begin_device(EfContext* ctx, const uint8_t* rgb_dev, const uint
     // ElasticFusion.cpp:302-323. The fill-in decision stays on the device: both candidate inputs are handed to the
     // pyramid kernels together with the flag.
     RC(map_dense_enough_async(ctx));
-    RC(map_select_model_inputs(ctx, nullptr, nullptr, nullptr));
+    RC(map_select_model_inputs(ctx));
     // initRGB's depth half (populateRGBDData -> verticesToDepth(vmaps_tmp), RGBDOdometry.cpp:212-222) reads the SAME
     // vmaps_tmp initICPModel just filled, so in frame-to-model mode nextDepth is identical to lastDepth: alias it for
     // the tracking call instead of building the pyramid twice.
@@ -1075,10 +917,10 @@ static int frame_begin_device(EfContext* ctx, const uint8_t* rgb_dev, const uint
     RC(odom_finish_async(ctx, 0, weight_multiplier, true));
   } else {
     CU(cudaStreamSynchronize(ctx->stream));
-    memcpy((char*)ctx->pin_small + 4096, in_T_wc, sizeof(double) * 16);
-    CU(cudaMemcpyAsync((char*)ctx->dev_small + 4096, (char*)ctx->pin_small + 4096, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+    memcpy(ctx->pin_small->T_wc, in_T_wc, sizeof(double) * 16);
+    CU(cudaMemcpyAsync(ctx->dev_small->T_wc, ctx->pin_small->T_wc, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
     ctx->so3_ready = false;  // no tracking for this frame: the SO(3) result of its input side is not used
-    RC(odom_set_pose_async(ctx, 0, (const double*)((char*)ctx->dev_small + 4096)));
+    RC(odom_set_pose_async(ctx, 0, ctx->dev_small->T_wc));
     RC(odom_finish_async(ctx, 0, weight_multiplier, false));
   }
   // (k_gn_finish also refreshed the map kernels' float pose + inverse from the new T_wc)
@@ -1101,7 +943,7 @@ static int frame_end_device(EfContext* ctx, int n_nodes, bool fern_accepted) {
     RC(map_predict_indices_async(ctx, ctx->tick, ctx->max_depth_processed, ctx->cfg.time_delta, 2));
     ef_stage(ctx, 9);
     if (n_nodes > 0 && !fern_accepted)  // ElasticFusion.cpp:559-569: the time-stamp refresh of deformed surfels reads this depth
-      RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick - ctx->cfg.time_delta, 65535, 2, false));
+      RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick - ctx->cfg.time_delta, 65535, 2));
     RC(map_clean_async(ctx, ctx->tick, ctx->confidence, ctx->cfg.time_delta, ctx->max_depth_processed, n_nodes, fern_accepted));
     ef_stage(ctx, 10);
   }
@@ -1121,6 +963,17 @@ extern "C" int ef_process_frame_device(EfContext* ctx, const uint8_t* rgb_dev, c
   return frame_end_device(ctx, 0, false);
 }
 
+// host frame -> pinned staging -> the live input textures, on ctx->stream
+static int stage_host_frame(EfContext* ctx, const uint8_t* rgb, const uint16_t* depth) {
+  const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
+  CU(cudaStreamSynchronize(ctx->stream));  // the staging buffers may still be in flight from the previous frame
+  memcpy(ctx->pin_rgb, rgb, n * 3);
+  memcpy(ctx->pin_depth, depth, n * 2);
+  CU(cudaMemcpyAsync(ctx->tex.rgb, ctx->pin_rgb, n * 3, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->tex.depth_raw, ctx->pin_depth, n * 2, cudaMemcpyHostToDevice, ctx->stream));
+  return 0;
+}
+
 // processFrame split at the point where the reference hands control to its CPU deformation solver (ElasticFusion.cpp:505-526):
 // begin = everything up to and including the local loop closure front half, end = fuse / clean / predict. Between the two
 // the host may read ef_local_loop_result, run Deformation::constrain (unchanged reference code) and hand its output back:
@@ -1130,12 +983,7 @@ extern "C" int ef_process_frame_begin(EfContext* ctx, const uint8_t* rgb, const 
   (void)timestamp;
   if (!ctx || !rgb || !depth) return EF_EINVAL;
   if (ctx->la.pending || ctx->frame_open) return EF_ESTATE;
-  const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
-  CU(cudaStreamSynchronize(ctx->stream));
-  memcpy(ctx->pin_rgb, rgb, n * 3);
-  memcpy(ctx->pin_depth, depth, n * 2);
-  CU(cudaMemcpyAsync(ctx->tex.rgb, ctx->pin_rgb, n * 3, cudaMemcpyHostToDevice, ctx->stream));
-  CU(cudaMemcpyAsync(ctx->tex.depth_raw, ctx->pin_depth, n * 2, cudaMemcpyHostToDevice, ctx->stream));
+  RC(stage_host_frame(ctx, rgb, depth));
   RC(frame_begin_device(ctx, ctx->tex.rgb, ctx->tex.depth_raw, weight_multiplier, in_T_wc));
   return ef_finish_frame(ctx);  // pose (and the loop-closure result) are final on return
 }
@@ -1218,12 +1066,12 @@ extern "C" int ef_join_lookahead(EfContext* ctx) {
 // Completes the frame enqueued by ef_process_frame_device: pose and surfel count are read back and final on return.
 extern "C" int ef_finish_frame(EfContext* ctx) {
   if (!ctx) return EF_EINVAL;
-  char* s = (char*)ctx->pin_small + 8192;
-  CU(cudaMemcpyAsync(s, (char*)ctx->odom[0].gn + offsetof(GNState, T_wc), sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(s + 128, ctx->map.count, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  PinStaging* s = ctx->pin_small;
+  CU(cudaMemcpyAsync(s->finish_T_wc, ctx->odom[0].gn->T_wc, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&s->finish_count, ctx->map.count, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  memcpy(ctx->T_wc, s, sizeof(double) * 16);
-  ctx->host_count = *(int*)(s + 128);
+  memcpy(ctx->T_wc, s->finish_T_wc, sizeof(double) * 16);
+  ctx->host_count = s->finish_count;
   return 0;
 }
 
@@ -1235,13 +1083,7 @@ extern "C" int ef_process_frame(EfContext* ctx, const uint8_t* rgb, const uint16
     return ef_finish_frame(ctx);
   }
   if (ctx->la.pending) return EF_ESTATE;  // a prefetched frame must be consumed first; nothing has been touched yet
-  const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
-  // the staging buffers may still be in flight from the previous frame
-  CU(cudaStreamSynchronize(ctx->stream));
-  memcpy(ctx->pin_rgb, rgb, n * 3);
-  memcpy(ctx->pin_depth, depth, n * 2);
-  CU(cudaMemcpyAsync(ctx->tex.rgb, ctx->pin_rgb, n * 3, cudaMemcpyHostToDevice, ctx->stream));
-  CU(cudaMemcpyAsync(ctx->tex.depth_raw, ctx->pin_depth, n * 2, cudaMemcpyHostToDevice, ctx->stream));
+  RC(stage_host_frame(ctx, rgb, depth));
   RC(ef_process_frame_device(ctx, ctx->tex.rgb, ctx->tex.depth_raw, timestamp, weight_multiplier, in_T_wc));
   // results the caller can observe (get_T_wc, counts) are final on return
   return ef_finish_frame(ctx);

@@ -11,8 +11,6 @@
 #include <math.h>
 #include <string.h>
 
-#include <vector>
-
 #include "ef_device.cuh"
 #include "ef_internal.h"
 
@@ -42,7 +40,7 @@ struct DeformWork {
   float* nodes16 = nullptr;
   double* rt12 = nullptr;                                 // R (column-major) and t of each node, fp64
   EfDeformResult* out = nullptr;
-  std::vector<void*> blocks;
+  Arena arena;  // every buffer above
 };
 
 struct Args {
@@ -571,50 +569,33 @@ __global__ void __launch_bounds__(THREADS) k_deform_solve(Args A) {
   }
 }
 
-template <typename T>
-cudaError_t grow(DeformWork* w, T** p, size_t n) {
-  void* q = nullptr;
-  cudaError_t e = cudaMalloc(&q, n * sizeof(T) + 256);
-  if (e != cudaSuccess) return e;
-  w->blocks.push_back(q);
-  *p = (T*)q;
-  return cudaSuccess;
-}
-
-#define DCU(x)                                 \
-  do {                                         \
-    cudaError_t e__ = (x);                     \
-    if (e__ != cudaSuccess) return (int)e__;   \
-  } while (0)
-
 // (re)allocates the workspace for n nodes and m constraints; never shrinks
 int reserve(DeformWork* w, int n, int m) {
   if (n <= w->cap_nodes && m <= w->cap_cons) return 0;
-  for (void* p : w->blocks) cudaFree(p);
-  w->blocks.clear();
+  w->arena.release();
   n = n > w->cap_nodes ? n : w->cap_nodes;
   m = m > w->cap_cons ? m : w->cap_cons;
-  DCU(grow(w, &w->pos, 3 * n));
-  DCU(grow(w, &w->ntime, n));
-  DCU(grow(w, &w->R, 9 * n));
-  DCU(grow(w, &w->t, 3 * n));
-  DCU(grow(w, &w->src, 3 * m));
-  DCU(grow(w, &w->dst, 3 * m));
-  DCU(grow(w, &w->ctime, m));
-  DCU(grow(w, &w->cnode, KNN * m));
-  DCU(grow(w, &w->cw, KNN * m));
-  DCU(grow(w, &w->list_off, n + 1));
-  DCU(grow(w, &w->list, KNN * m));
-  DCU(grow(w, &w->res_rot, 6 * n));
-  DCU(grow(w, &w->res_reg, 3 * NB * n));
-  DCU(grow(w, &w->res_con, 3 * m));
-  DCU(grow(w, &w->cerr, m));
-  DCU(grow(w, &w->band, (size_t)n * (MAXBW + 1) * 144));
-  DCU(grow(w, &w->linv, (size_t)n * 144));
-  DCU(grow(w, &w->x, (size_t)n * NV));
-  DCU(grow(w, &w->nodes16, 16 * n));
-  DCU(grow(w, &w->rt12, 12 * n));
-  DCU(grow(w, &w->out, 1));
+  CU(w->arena.alloc(&w->pos, 3 * n));
+  CU(w->arena.alloc(&w->ntime, n));
+  CU(w->arena.alloc(&w->R, 9 * n));
+  CU(w->arena.alloc(&w->t, 3 * n));
+  CU(w->arena.alloc(&w->src, 3 * m));
+  CU(w->arena.alloc(&w->dst, 3 * m));
+  CU(w->arena.alloc(&w->ctime, m));
+  CU(w->arena.alloc(&w->cnode, KNN * m));
+  CU(w->arena.alloc(&w->cw, KNN * m));
+  CU(w->arena.alloc(&w->list_off, n + 1));
+  CU(w->arena.alloc(&w->list, KNN * m));
+  CU(w->arena.alloc(&w->res_rot, 6 * n));
+  CU(w->arena.alloc(&w->res_reg, 3 * NB * n));
+  CU(w->arena.alloc(&w->res_con, 3 * m));
+  CU(w->arena.alloc(&w->cerr, m));
+  CU(w->arena.alloc(&w->band, (size_t)n * (MAXBW + 1) * 144));
+  CU(w->arena.alloc(&w->linv, (size_t)n * 144));
+  CU(w->arena.alloc(&w->x, (size_t)n * NV));
+  CU(w->arena.alloc(&w->nodes16, 16 * n));
+  CU(w->arena.alloc(&w->rt12, 12 * n));
+  CU(w->arena.alloc(&w->out, 1));
   w->cap_nodes = n;
   w->cap_cons = m;
   return 0;
@@ -625,7 +606,7 @@ int reserve(DeformWork* w, int n, int m) {
 void deform_free(EfContext* ctx) {
   DeformWork* w = static_cast<DeformWork*>(ctx->deform);
   if (!w) return;
-  for (void* p : w->blocks) cudaFree(p);
+  w->arena.release();
   delete w;
   ctx->deform = nullptr;
 }
@@ -636,13 +617,13 @@ int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_ti
                  int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out) {
   if (!ctx->deform) ctx->deform = new DeformWork();
   DeformWork* w = static_cast<DeformWork*>(ctx->deform);
-  if (int rc = reserve(w, n, m)) return rc;
+  RC(reserve(w, n, m));
   cudaStream_t st = ctx->stream;
-  DCU(cudaMemcpyAsync(w->pos, node_pos3, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, st));
-  DCU(cudaMemcpyAsync(w->ntime, node_times, sizeof(int) * n, cudaMemcpyHostToDevice, st));
-  DCU(cudaMemcpyAsync(w->src, src3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
-  DCU(cudaMemcpyAsync(w->dst, dst3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
-  DCU(cudaMemcpyAsync(w->ctime, src_times, sizeof(int) * m, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->pos, node_pos3, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->ntime, node_times, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->src, src3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->dst, dst3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->ctime, src_times, sizeof(int) * m, cudaMemcpyHostToDevice, st));
   Args a;
   a.n = n;
   a.m = m;
@@ -659,13 +640,13 @@ int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_ti
   a.rt12 = w->rt12;
   a.out = w->out;
   EF_LAUNCH(ctx, k_deform_solve, 1, THREADS, 0, a);
-  DCU(cudaGetLastError());
-  DCU(cudaMemcpyAsync(out, w->out, sizeof(EfDeformResult), cudaMemcpyDeviceToHost, st));
-  if (nodes16_host) DCU(cudaMemcpyAsync(nodes16_host, w->nodes16, sizeof(float) * 16 * n, cudaMemcpyDeviceToHost, st));
-  if (rt12_host) DCU(cudaMemcpyAsync(rt12_host, w->rt12, sizeof(double) * 12 * n, cudaMemcpyDeviceToHost, st));
-  if (cons_nodes4) DCU(cudaMemcpyAsync(cons_nodes4, w->cnode, sizeof(int) * KNN * m, cudaMemcpyDeviceToHost, st));
-  if (cons_weights4) DCU(cudaMemcpyAsync(cons_weights4, w->cw, sizeof(double) * KNN * m, cudaMemcpyDeviceToHost, st));
-  DCU(cudaStreamSynchronize(st));
+  CHECK_LAST();
+  CU(cudaMemcpyAsync(out, w->out, sizeof(EfDeformResult), cudaMemcpyDeviceToHost, st));
+  if (nodes16_host) CU(cudaMemcpyAsync(nodes16_host, w->nodes16, sizeof(float) * 16 * n, cudaMemcpyDeviceToHost, st));
+  if (rt12_host) CU(cudaMemcpyAsync(rt12_host, w->rt12, sizeof(double) * 12 * n, cudaMemcpyDeviceToHost, st));
+  if (cons_nodes4) CU(cudaMemcpyAsync(cons_nodes4, w->cnode, sizeof(int) * KNN * m, cudaMemcpyDeviceToHost, st));
+  if (cons_weights4) CU(cudaMemcpyAsync(cons_weights4, w->cw, sizeof(double) * KNN * m, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   return 0;
 }
 

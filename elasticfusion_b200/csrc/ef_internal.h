@@ -1,7 +1,10 @@
-// Internal context layout of libefusion.so (not part of the ABI).
+// Internal context layout of libefusion.so (not part of the ABI) and the host-side plumbing every translation unit shares:
+// allocation, error macros, the launch helper and the entry points one .cu file calls in another.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <vector>
 
 #include "../../include/efusion_b200.h"
 
@@ -209,6 +212,41 @@ struct Lookahead {
   uint16_t* pin_depth;
 };
 
+// Device buffers owned by one context (or one workspace), freed together. Every block has 256 bytes of slack.
+struct Arena {
+  std::vector<void*> blocks;
+  template <typename T>
+  cudaError_t alloc(T** p, size_t n) {
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, n * sizeof(T) + 256);
+    if (e != cudaSuccess) return e;
+    blocks.push_back(q);
+    *p = (T*)q;
+    return cudaSuccess;
+  }
+  void release() {
+    for (void* p : blocks) cudaFree(p);
+    blocks.clear();
+  }
+};
+
+// Layout of the pinned staging block (EfContext::pin_small): host values on their way to the device and results on their way
+// back. A slot is rewritten only after a cudaStreamSynchronize, since a copy enqueued by the previous call may still read it.
+struct PinStaging {
+  float icp_inputs[36];  // ef_icp_step_async: Rcurr, tcurr, Rprev_inv, tprev, then M = R_prev^-1 R_curr, t' (9 + 3 each)
+  double map_pose[16];   // map_update_pose_async: T_wc of a stage-API map call
+  float weighting;       // map_fuse_async: fusion weighting of a stage-API fuse
+  double T_wc[16];       // frame_begin_device: the caller's pose for a frame that is not tracked
+  double finish_T_wc[16];  // ef_finish_frame: pose and surfel count read back
+  int finish_count;
+};
+// Layout of the device staging block (EfContext::dev_small): where the kernels read the pinned slots above.
+struct DevStaging {
+  double map_pose[16];
+  double T_wc[16];
+};
+static_assert(sizeof(PinStaging) <= 65536 && sizeof(DevStaging) <= 65536, "staging blocks stay within 64 KiB");
+
 }  // namespace ef
 
 struct EfContext {
@@ -249,11 +287,35 @@ struct EfContext {
   // pinned staging
   uint8_t* pin_rgb;
   uint16_t* pin_depth;
-  void* pin_small;   // results read-back
-  void* dev_small;   // upload area for per-call parameters
+  ef::PinStaging* pin_small;  // per-call parameters and results read-back
+  ef::DevStaging* dev_small;  // device side of the per-call parameters
   void* map_host;    // host-side bookkeeping of the surfel buffers (ef_map.cu)
   void* deform;      // workspace of the deformation-graph solve (ef_deform.cu), allocated by its first call
+  ef::Arena arena;   // every device buffer of the context
 };
+
+// error propagation of the host entry points: a CUDA error code, or the code of a failed internal call
+#define CU(x)                                  \
+  do {                                         \
+    cudaError_t e__ = (x);                     \
+    if (e__ != cudaSuccess) return (int)e__;   \
+  } while (0)
+#define RC(x)              \
+  do {                     \
+    int rc__ = (x);        \
+    if (rc__) return rc__; \
+  } while (0)
+#define CHECK_LAST() CU(cudaGetLastError())
+
+namespace ef {
+// n elements of T from the context's arena; fill >= 0: every byte set to `fill` on ctx->stream
+template <typename T>
+inline cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n, int fill = -1) {
+  cudaError_t e = ctx->arena.alloc(p, n);
+  if (e != cudaSuccess || fill < 0) return e;
+  return cudaMemsetAsync(*p, fill, n * sizeof(T), ctx->stream);
+}
+}  // namespace ef
 
 // launch bookkeeping
 inline void ef_stage(EfContext* ctx, int i) {
@@ -263,25 +325,99 @@ inline void ef_stage(EfContext* ctx, int i) {
     ctx->stage_n |= 1 << i;
   }
 }
+inline cudaLaunchAttribute cluster_attr(int cluster) {
+  cudaLaunchAttribute a;
+  a.id = cudaLaunchAttributeClusterDimension;
+  a.val.clusterDim.x = cluster;
+  a.val.clusterDim.y = 1;
+  a.val.clusterDim.z = 1;
+  return a;
+}
 // Every kernel is launched with programmatic stream serialisation allowed (see pdl_enter() in ef_device.cuh); set
 // EF_NO_PDL=1 in the environment to fall back to plain stream-ordered launches (A/B measurements).
+// cluster > 0: the grid runs as thread-block clusters of that many CTAs.
 template <typename... KArgs, typename... Args>
-inline void ef_launch(EfContext* ctx, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
+inline void ef_launch(EfContext* ctx, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, int cluster, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = ctx->stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (cluster > 0) attr[n++] = cluster_attr(cluster);
+  if (ctx->pdl && !ctx->plain_next) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = (ctx->pdl && !ctx->plain_next) ? 1 : 0;
+  cfg.numAttrs = n;
   ctx->plain_next = false;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
   ctx->launches++;
 }
-#define EF_LAUNCH(ctx, kernel, grid, block, smem, ...) ef_launch((ctx), kernel, dim3(grid), dim3(block), (smem), __VA_ARGS__)
+#define EF_LAUNCH(ctx, kernel, grid, block, smem, ...) ef_launch((ctx), kernel, dim3(grid), dim3(block), (smem), 0, __VA_ARGS__)
 // the next launch is a plain stream-ordered one: it starts only after everything enqueued before it has completed, so no
 // kernel launched after it can become resident while earlier work is still running (a full barrier in the PDL chain)
 #define EF_PLAIN_NEXT(ctx) ((ctx)->plain_next = true)
+
+// grid of a grid-stride kernel over n items: ceil(n / threads) CTAs, at least one, at most one wave of per_sm per SM
+inline int wave_blocks(const EfContext* ctx, size_t n, int per_sm = 8, int threads = 256) {
+  size_t b = (n + threads - 1) / threads, cap = (size_t)ctx->num_sms * per_sm;
+  return (int)(b < cap ? (b ? b : 1) : cap);
+}
+
+// ---- host entry points one translation unit calls in another; default arguments live here only -------------------
+namespace ef {
+// ef_track.cu: the tracker's input pyramids
+int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff);
+int odom_init_icp_pred(EfContext* ctx, int which, const float* vtx4, const float* nrm4);
+int odom_init_icp_model(EfContext* ctx, int which, const float* vtx4, const float* nrm4, bool with_global = true);
+int odom_populate(EfContext* ctx, int which, const uint8_t* rgba, float** destDepths, uint8_t** destImages, bool with_depth,
+                  bool with_image = true);
+int map_select_model_inputs(EfContext* ctx);
+int launch_sobel(EfContext* ctx, int which);
+
+// ef_reduce.cu: SO(3) loop, Gauss-Newton schedule and the stage API's reductions
+int odom_cluster_size(int want);
+int odom_so3_async(EfContext* ctx, int which);
+int odom_track_async(EfContext* ctx, int which, bool rgbOnly, float icpWeight, bool pyramid, bool fastOdom, bool so3);
+int odom_finish_async(EfContext* ctx, int which, float weightMultiplier, bool have_track);
+int odom_set_pose_async(EfContext* ctx, int which, const double* T_dev);
+int launch_se3_step_raw(EfContext* ctx, int which, int level, bool do_icp, bool do_rgb, float sigma);
+int launch_rgb_residual_raw(EfContext* ctx, int which, int level);
+int launch_icp_dense_only(EfContext* ctx, int which, int level);
+int launch_so3_raw(EfContext* ctx, int which);
+
+// ef_preprocess.cu
+int preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric, float* metric_filtered);
+int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba);
+
+// ef_map.cu: the surfel map
+int alloc_map(EfContext* ctx);
+void map_free_host(EfContext* ctx);
+int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_b, size_t max_items, int* offsets, int* total);
+void scan_scratch(EfContext* ctx, uint8_t** flags, int** offsets);
+int map_initialise_async(EfContext* ctx);
+int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
+int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, int time_delta, int vis_mode = 0);
+int map_fuse_async(EfContext* ctx, int time_or_neg, float max_depth, float weighting_or_neg);
+int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0, bool is_fern = false);
+int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);
+int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode);
+int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
+int map_dense_enough_async(EfContext* ctx);
+int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
+int map_loop_reset_async(EfContext* ctx);
+int odom_copy_pose_async(EfContext* ctx, int dst, int src);
+int map_download(EfContext* ctx, const float4* a, const float4* b, const float4* c, int n, float* out);
+int map_upload(EfContext* ctx, const float* in, int n);
+int map_upload_range(EfContext* ctx, const float* in, int first, int n);
+int map_resize_to_host(EfContext* ctx, const void* src_dev, int elem, int factor, void* host_out);
+
+// ef_deform.cu: the deformation-graph solve
+int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
+                 const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
+                 int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out);
+void deform_free(EfContext* ctx);
+}  // namespace ef

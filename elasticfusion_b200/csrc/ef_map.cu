@@ -19,11 +19,6 @@
 
 using namespace ef;
 
-namespace ef {
-template <typename T>
-cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n);
-}
-
 namespace {
 
 constexpr unsigned long long kEmptyKey = ~0ull;
@@ -1375,24 +1370,9 @@ __global__ void k_unpack_aos(const float4* __restrict__ in, int n, float4* __res
   }
 }
 
-inline int sblocks(const EfContext* ctx, size_t n, int per_sm = 8, int threads = 256) {
-  size_t b = (n + threads - 1) / threads, cap = (size_t)ctx->num_sms * per_sm;
-  return (int)(b < cap ? (b ? b : 1) : cap);
-}
 inline Cam cam_of(const EfContext* ctx) { return Cam{ctx->cfg.cx, ctx->cfg.cy, ctx->cfg.fx, ctx->cfg.fy}; }
 
 }  // namespace
-
-#define CU(x)                                \
-  do {                                       \
-    cudaError_t e__ = (x);                   \
-    if (e__ != cudaSuccess) return (int)e__; \
-  } while (0)
-#define LAST()                                \
-  do {                                        \
-    cudaError_t e__ = cudaGetLastError();     \
-    if (e__ != cudaSuccess) return (int)e__;  \
-  } while (0)
 
 struct MapBuffers {
   int *offsets;
@@ -1400,7 +1380,7 @@ struct MapBuffers {
   int *fb_off_raw, *fb_off_filt;
   uint8_t *fb_flag_raw, *fb_flag_filt;
   float4* aos;  // staging for download/upload
-  size_t aos_cap;
+  size_t aos_bytes;
   unsigned int scan_epoch;  // tag of the current scan's tile states (k_scan_flags)
   size_t scan_state_bytes;
 };
@@ -1408,6 +1388,26 @@ struct MapBuffers {
 namespace ef {
 
 static MapBuffers& mb(EfContext* ctx) { return *reinterpret_cast<MapBuffers*>(ctx->map_host); }
+
+// grows the AoS staging buffer to at least `bytes` (never shrinks)
+static int aos_reserve(MapBuffers& B, size_t bytes) {
+  if (bytes <= B.aos_bytes) return 0;
+  if (B.aos) cudaFree(B.aos);
+  B.aos = nullptr;
+  B.aos_bytes = 0;
+  CU(cudaMalloc((void**)&B.aos, bytes));
+  B.aos_bytes = bytes;
+  return 0;
+}
+
+// next tag of the look-back tile states (k_scan_flags, k_clean_move)
+static int next_scan_epoch(EfContext* ctx, MapBuffers& B) {
+  if (++B.scan_epoch >= (1u << 30)) {  // epoch field exhausted (never in practice): start over with clean states
+    CU(cudaMemsetAsync(ctx->map.scan_tile_state, 0, B.scan_state_bytes, ctx->stream));
+    B.scan_epoch = 1;
+  }
+  return 0;
+}
 
 int alloc_map(EfContext* ctx) {
   MapDev& m = ctx->map;
@@ -1431,56 +1431,46 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &m.norm_rad, cap));
   CU(cudaFuncSetAttribute(k_clean_move<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CcShared)));
   CU(cudaFuncSetAttribute(k_clean_move<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CcShared)));
-  CU(ctx_alloc(ctx, &m.count, 4));
+  CU(ctx_alloc(ctx, &m.count, 4, 0));
   CU(ctx_alloc(ctx, &m.new_pos, n));
   CU(ctx_alloc(ctx, &m.new_col, n));
   CU(ctx_alloc(ctx, &m.new_nr, n));
-  CU(ctx_alloc(ctx, &m.new_count, 4));
+  CU(ctx_alloc(ctx, &m.new_count, 4, 0));
   CU(ctx_alloc(ctx, &m.assoc_id, n));
-  CU(ctx_alloc(ctx, &m.pending, cap));
-  CU(ctx_alloc(ctx, &m.zbuf, n));
+  CU(ctx_alloc(ctx, &m.pending, cap, 0xff));
+  CU(ctx_alloc(ctx, &m.zbuf, n, 0xff));  // kept cleared by the resolve passes from here on
   // look-back tile states: the clean pass walks capacity + n surfels in tiles of CC_TILE, the image-sized compactions
   // (first-frame feedback, new surfels, the tracker's candidate list) <= 2 n items in tiles of SCAN_TILE
   const size_t max_items = cap + n;
   const size_t tiles = (max_items + CC_TILE - 1) / CC_TILE + (2 * n + SCAN_TILE - 1) / SCAN_TILE + 2;
   unsigned long long* st = nullptr;
-  CU(ctx_alloc(ctx, &st, tiles));
+  CU(ctx_alloc(ctx, &st, tiles, 0));
   m.scan_tile_state = reinterpret_cast<int*>(st);
-  CU(ctx_alloc(ctx, &m.scan_counter, 4));
+  CU(ctx_alloc(ctx, &m.scan_counter, 4, 0));
   CU(ctx_alloc(ctx, &m.clean_ctl, 4));
+  CU(cudaMemsetAsync(m.clean_ctl, 0, 8, ctx->stream));
+  CU(cudaMemsetAsync(m.clean_ctl + 2, 0xff, 8, ctx->stream));
   CU(ctx_alloc(ctx, &m.vis_list, cap));
-  CU(ctx_alloc(ctx, &m.vis_count, 4));
-  CU(cudaMemsetAsync(m.vis_count, 0, 16, ctx->stream));
+  CU(ctx_alloc(ctx, &m.vis_count, 4, 0));
   CU(ctx_alloc(ctx, &m.keep_mask, ((max_items + CC_TILE - 1) / CC_TILE) * CC_WORDS));
   CU(ctx_alloc(ctx, &m.flags, 2 * n));
   CU(ctx_alloc(ctx, &B->offsets, 2 * n));
-  CU(ctx_alloc(ctx, &B->totals, 4));
+  CU(ctx_alloc(ctx, &B->totals, 4, 0));
   CU(ctx_alloc(ctx, &B->fb_off_raw, n));
   CU(ctx_alloc(ctx, &B->fb_off_filt, n));
   CU(ctx_alloc(ctx, &B->fb_flag_raw, n));
   CU(ctx_alloc(ctx, &B->fb_flag_filt, n));
   CU(ctx_alloc(ctx, &m.pose, 1));
-  CU(ctx_alloc(ctx, &m.dense_flag, 4));
+  CU(ctx_alloc(ctx, &m.dense_flag, 4, 0));
   CU(ctx_alloc(ctx, &m.tick, 4));
   CU(ctx_alloc(ctx, &m.nodes, (size_t)MAX_GRAPH_NODES * 16));
-  CU(ctx_alloc(ctx, &m.loop, 1));
-  CU(cudaMemsetAsync(m.loop, 0, sizeof(LoopDev), ctx->stream));
+  CU(ctx_alloc(ctx, &m.loop, 1, 0));
   m.loop_capacity = loop_constraint_capacity(c.width, c.height);
   CU(ctx_alloc(ctx, &m.loop_src, (size_t)m.loop_capacity * 3));
   CU(ctx_alloc(ctx, &m.loop_dst, (size_t)m.loop_capacity * 3));
   CU(ctx_alloc(ctx, &m.loop_times, (size_t)m.loop_capacity));
   B->scan_epoch = 0;
   B->scan_state_bytes = tiles * 8;
-  CU(cudaMemsetAsync(m.scan_tile_state, 0, tiles * 8, ctx->stream));
-  CU(cudaMemsetAsync(m.scan_counter, 0, 16, ctx->stream));
-  CU(cudaMemsetAsync(m.clean_ctl, 0, 8, ctx->stream));
-  CU(cudaMemsetAsync(m.clean_ctl + 2, 0xff, 8, ctx->stream));
-  CU(cudaMemsetAsync(m.zbuf, 0xff, n * 8, ctx->stream));  // kept cleared by the resolve passes from here on
-  CU(cudaMemsetAsync(m.count, 0, 16, ctx->stream));
-  CU(cudaMemsetAsync(m.new_count, 0, 16, ctx->stream));
-  CU(cudaMemsetAsync(m.pending, 0xff, cap * 4, ctx->stream));
-  CU(cudaMemsetAsync(m.dense_flag, 0, 16, ctx->stream));
-  CU(cudaMemsetAsync(B->totals, 0, 16, ctx->stream));
   const int one = 1;
   CU(cudaMemcpyAsync(m.tick, &one, 4, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1491,14 +1481,11 @@ int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_
   MapDev& m = ctx->map;
   const size_t tiles = (max_items + SCAN_TILE - 1) / SCAN_TILE + 1;
   MapBuffers& B = mb(ctx);
-  if (++B.scan_epoch >= (1u << 30)) {  // epoch field exhausted (never in practice): start over with clean states
-    CU(cudaMemsetAsync(m.scan_tile_state, 0, B.scan_state_bytes, ctx->stream));
-    B.scan_epoch = 1;
-  }
+  RC(next_scan_epoch(ctx, B));
   size_t nb = tiles < (size_t)ctx->num_sms * 4 ? tiles : (size_t)ctx->num_sms * 4;
   EF_LAUNCH(ctx, k_scan_flags, (int)nb, SCAN_THREADS, 0, flags, n_a, n_b, offsets, (unsigned long long*)m.scan_tile_state, m.scan_counter, total,
             B.scan_epoch);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1507,12 +1494,12 @@ int map_update_pose_async(EfContext* ctx, const double* T_host) {
   const double* src = ctx->odom[0].gn->T_wc;
   if (T_host) {
     CU(cudaStreamSynchronize(ctx->stream));
-    memcpy((char*)ctx->pin_small + 1024, T_host, sizeof(double) * 16);
-    CU(cudaMemcpyAsync((char*)ctx->dev_small + 1024, (char*)ctx->pin_small + 1024, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
-    src = (const double*)((char*)ctx->dev_small + 1024);
+    memcpy(ctx->pin_small->map_pose, T_host, sizeof(double) * 16);
+    CU(cudaMemcpyAsync(ctx->dev_small->map_pose, ctx->pin_small->map_pose, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+    src = ctx->dev_small->map_pose;
   }
   EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, ctx->map.pose, src);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1520,20 +1507,18 @@ int map_initialise_async(EfContext* ctx) {
   MapDev& m = ctx->map;
   MapBuffers& B = mb(ctx);
   const int n = m.rows * m.cols;
-  EF_LAUNCH(ctx, k_feedback_flags, sblocks(ctx, n), 256, 0, ctx->tex.depth_metric, ctx->tex.depth_metric_filtered, m.rows, m.cols,
+  EF_LAUNCH(ctx, k_feedback_flags, wave_blocks(ctx, n), 256, 0, ctx->tex.depth_metric, ctx->tex.depth_metric_filtered, m.rows, m.cols,
             ctx->max_depth_processed, B.fb_flag_raw, B.fb_flag_filt);
   // device-resident element count for the scans: reuse new_count as "n pixels"
   EF_LAUNCH(ctx, k_set_int, 1, 32, 0, m.new_count, n);
-  int rc = run_scan(ctx, B.fb_flag_raw, m.new_count, nullptr, n, B.fb_off_raw, B.totals + 0);
-  if (rc) return rc;
-  rc = run_scan(ctx, B.fb_flag_filt, m.new_count, nullptr, n, B.fb_off_filt, B.totals + 1);
-  if (rc) return rc;
+  RC(run_scan(ctx, B.fb_flag_raw, m.new_count, nullptr, n, B.fb_off_raw, B.totals + 0));
+  RC(run_scan(ctx, B.fb_flag_filt, m.new_count, nullptr, n, B.fb_off_filt, B.totals + 1));
   CU(cudaMemsetAsync(m.norm_rad, 0, (size_t)(n < m.capacity ? n : m.capacity) * sizeof(float4), ctx->stream));
-  EF_LAUNCH(ctx, k_init_scatter, sblocks(ctx, n), 256, 0, ctx->tex.rgb, ctx->tex.depth_metric, ctx->tex.depth_metric_filtered, m.rows, m.cols,
+  EF_LAUNCH(ctx, k_init_scatter, wave_blocks(ctx, n), 256, 0, ctx->tex.rgb, ctx->tex.depth_metric, ctx->tex.depth_metric_filtered, m.rows, m.cols,
             cam_of(ctx), ctx->tick, B.fb_flag_raw, B.fb_flag_filt, B.fb_off_raw, B.fb_off_filt, B.totals + 0, m.capacity, m.pos_conf,
             m.color_time, m.norm_rad, m.count);
   EF_LAUNCH(ctx, k_set_int, 1, 32, 0, m.new_count, 0);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1557,9 +1542,9 @@ int map_predict_indices_async(EfContext* ctx, int time, float max_depth, int tim
   else
     EF_LAUNCH(ctx, k_index_scatter<0>, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols,
               cam_of(ctx), m.zbuf, (uint32_t*)nullptr, (int*)nullptr, 0);
-  EF_LAUNCH(ctx, k_index_resolve, sblocks(ctx, n), 256, 0, m.pos_conf, m.color_time, m.norm_rad, m.pose, n, m.zbuf, ctx->tex.index,
+  EF_LAUNCH(ctx, k_index_resolve, wave_blocks(ctx, n), 256, 0, m.pos_conf, m.color_time, m.norm_rad, m.pose, n, m.zbuf, ctx->tex.index,
             ctx->tex.vert_conf, ctx->tex.color_time, ctx->tex.norm_rad, vis_mode == 2 ? m.vis_count : (int*)nullptr);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1583,23 +1568,20 @@ static FuseArgs fuse_args(EfContext* ctx, int time, float max_depth) {
 int map_fuse_async(EfContext* ctx, int time, float max_depth, float weighting) {
   MapDev& m = ctx->map;
   MapBuffers& B = mb(ctx);
-  const int n = m.rows * m.cols;
   if (weighting >= 0) {
     CU(cudaStreamSynchronize(ctx->stream));
-    *(float*)((char*)ctx->pin_small + 2048) = weighting;
-    CU(cudaMemcpyAsync((char*)ctx->odom[0].gn + offsetof(GNState, weighting), (char*)ctx->pin_small + 2048, 4, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->pin_small->weighting = weighting;
+    CU(cudaMemcpyAsync(&ctx->odom[0].gn->weighting, &ctx->pin_small->weighting, 4, cudaMemcpyHostToDevice, ctx->stream));
   }
   FuseArgs a = fuse_args(ctx, time, max_depth);
   const Quarter Q = quarter_of(time, m.rows, m.cols);
   const int nq = Q.ni * Q.nj;
-  (void)n;
-  EF_LAUNCH(ctx, k_fuse_associate, sblocks(ctx, nq, 16, 128), 128, 0, a, m.count, m.assoc_id, m.pending, m.flags);
+  EF_LAUNCH(ctx, k_fuse_associate, wave_blocks(ctx, nq, 16, 128), 128, 0, a, m.count, m.assoc_id, m.pending, m.flags);
   EF_LAUNCH(ctx, k_set_int, 1, 32, 0, m.new_count, nq);
-  int rc = run_scan(ctx, m.flags, m.new_count, nullptr, nq, B.offsets, B.totals + 2);
-  if (rc) return rc;
-  EF_LAUNCH(ctx, k_fuse_update, sblocks(ctx, nq, 16, 128), 128, 0, a, m.pose, (const GNState*)ctx->odom[0].gn, m.count, m.assoc_id, m.pending, B.offsets,
+  RC(run_scan(ctx, m.flags, m.new_count, nullptr, nq, B.offsets, B.totals + 2));
+  EF_LAUNCH(ctx, k_fuse_update, wave_blocks(ctx, nq, 16, 128), 128, 0, a, m.pose, (const GNState*)ctx->odom[0].gn, m.count, m.assoc_id, m.pending, B.offsets,
             B.totals + 2, m.pos_conf, m.color_time, m.norm_rad, m.new_pos, m.new_col, m.new_nr, m.new_count);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1625,10 +1607,7 @@ int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_del
   // test (parallel) -> order-preserving in-place compaction + append of the new surfels + count publication (movers only)
   const size_t max_items = (size_t)m.capacity + (size_t)m.rows * m.cols;
   const size_t tiles = (max_items + CC_TILE - 1) / CC_TILE;
-  if (++B.scan_epoch >= (1u << 30)) {
-    CU(cudaMemsetAsync(m.scan_tile_state, 0, B.scan_state_bytes, ctx->stream));
-    B.scan_epoch = 1;
-  }
+  RC(next_scan_epoch(ctx, B));
   // grids never depend on a surfel count the host would have to read back: the test strides over the tiles, the movers draw
   // tiles from a dispenser (one resident wave: four 49 KB CTAs per SM)
   size_t nb = (size_t)ctx->num_sms * 4;
@@ -1647,11 +1626,11 @@ int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_del
     EF_LAUNCH(ctx, k_clean_move<false>, (int)nb, CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
               m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
               B.scan_epoch);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
-int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode, bool) {
+int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode) {
   MapDev& m = ctx->map;
   const int n = m.rows * m.cols;
   RayArgs a;
@@ -1666,15 +1645,15 @@ int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int
   EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.zbuf);
   Textures& t = ctx->tex;
   if (mode == 0)
-    EF_LAUNCH(ctx, k_splat_resolve, sblocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.image, t.vertex, t.normal,
+    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.image, t.vertex, t.normal,
               t.time, (float*)nullptr);
   else if (mode == 1)
-    EF_LAUNCH(ctx, k_splat_resolve, sblocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.old_image, t.old_vertex,
+    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.old_image, t.old_vertex,
               t.old_normal, t.old_time, (float*)nullptr);
   else
-    EF_LAUNCH(ctx, k_splat_resolve, sblocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, (uchar4*)nullptr,
+    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, (uchar4*)nullptr,
               (float4*)nullptr, (float4*)nullptr, (uint16_t*)nullptr, t.synth_depth);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -1682,29 +1661,24 @@ int map_fill_in_async(EfContext* ctx, bool pass_geom, bool pass_img) {
   MapDev& m = ctx->map;
   Textures& t = ctx->tex;
   const int n = m.rows * m.cols;
-  EF_LAUNCH(ctx, k_fill_in, sblocks(ctx, n), 256, 0, t.vertex, t.normal, t.image, t.depth_filtered, t.rgb, m.rows, m.cols, cam_of(ctx),
+  EF_LAUNCH(ctx, k_fill_in, wave_blocks(ctx, n), 256, 0, t.vertex, t.normal, t.image, t.depth_filtered, t.rgb, m.rows, m.cols, cam_of(ctx),
             pass_geom ? 1 : 0, pass_img ? 1 : 0, t.fill_vertex, t.fill_normal, t.fill_image);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
 int map_dense_enough_async(EfContext* ctx) {
   MapDev& m = ctx->map;
   EF_LAUNCH(ctx, k_dense_enough, 1, 256, 0, ctx->tex.image, m.rows, m.cols, 20, m.dense_flag);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
 int map_download(EfContext* ctx, const float4* a, const float4* b, const float4* c, int n, float* out) {
   MapBuffers& B = mb(ctx);
   if (n <= 0) return 0;
-  if ((size_t)n > B.aos_cap) {
-    if (B.aos) cudaFree(B.aos);
-    B.aos = nullptr;
-    CU(cudaMalloc((void**)&B.aos, (size_t)n * 48));
-    B.aos_cap = n;
-  }
-  EF_LAUNCH(ctx, k_pack_aos, sblocks(ctx, n), 256, 0, a, b, c, n, B.aos);
+  RC(aos_reserve(B, (size_t)n * 48));
+  EF_LAUNCH(ctx, k_pack_aos, wave_blocks(ctx, n), 256, 0, a, b, c, n, B.aos);
   CU(cudaMemcpyAsync(out, B.aos, (size_t)n * 48, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
@@ -1715,14 +1689,9 @@ int map_upload(EfContext* ctx, const float* in, int n) {
   MapBuffers& B = mb(ctx);
   if (n > m.capacity) return EF_EINVAL;
   if (n > 0) {
-    if ((size_t)n > B.aos_cap) {
-      if (B.aos) cudaFree(B.aos);
-      B.aos = nullptr;
-      CU(cudaMalloc((void**)&B.aos, (size_t)n * 48));
-      B.aos_cap = n;
-    }
+    RC(aos_reserve(B, (size_t)n * 48));
     CU(cudaMemcpyAsync(B.aos, in, (size_t)n * 48, cudaMemcpyHostToDevice, ctx->stream));
-    EF_LAUNCH(ctx, k_unpack_aos, sblocks(ctx, n), 256, 0, (const float4*)B.aos, n, m.pos_conf, m.color_time, m.norm_rad);
+    EF_LAUNCH(ctx, k_unpack_aos, wave_blocks(ctx, n), 256, 0, (const float4*)B.aos, n, m.pos_conf, m.color_time, m.norm_rad);
   }
   EF_LAUNCH(ctx, k_set_int, 1, 32, 0, m.count, n);
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1738,14 +1707,9 @@ int map_upload_range(EfContext* ctx, const float* in, int first, int n) {
   CU(cudaMemcpyAsync(&cnt, m.count, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if ((long long)first + n > cnt) return EF_EINVAL;
-  if ((size_t)n > B.aos_cap) {
-    if (B.aos) cudaFree(B.aos);
-    B.aos = nullptr;
-    CU(cudaMalloc((void**)&B.aos, (size_t)n * 48));
-    B.aos_cap = n;
-  }
+  RC(aos_reserve(B, (size_t)n * 48));
   CU(cudaMemcpyAsync(B.aos, in, (size_t)n * 48, cudaMemcpyHostToDevice, ctx->stream));
-  EF_LAUNCH(ctx, k_unpack_aos, sblocks(ctx, n), 256, 0, (const float4*)B.aos, n, m.pos_conf + first, m.color_time + first, m.norm_rad + first);
+  EF_LAUNCH(ctx, k_unpack_aos, wave_blocks(ctx, n), 256, 0, (const float4*)B.aos, n, m.pos_conf + first, m.color_time + first, m.norm_rad + first);
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
@@ -1773,13 +1737,8 @@ int map_resize_to_host(EfContext* ctx, const void* src_dev, int elem, int factor
   MapBuffers& B = mb(ctx);
   if (factor < 1 || m.rows / factor < 1 || m.cols / factor < 1) return EF_EINVAL;
   const size_t n = (size_t)(m.rows / factor) * (m.cols / factor);
-  if (n * elem > B.aos_cap * 48) {
-    if (B.aos) cudaFree(B.aos);
-    B.aos = nullptr;
-    CU(cudaMalloc((void**)&B.aos, n * elem + 48));
-    B.aos_cap = (n * elem + 47) / 48;
-  }
-  EF_LAUNCH(ctx, k_resize_nearest, sblocks(ctx, n), 256, 0, (const uint8_t*)src_dev, m.rows, m.cols, factor, elem, (uint8_t*)B.aos);
+  RC(aos_reserve(B, n * elem));
+  EF_LAUNCH(ctx, k_resize_nearest, wave_blocks(ctx, n), 256, 0, (const uint8_t*)src_dev, m.rows, m.cols, factor, elem, (uint8_t*)B.aos);
   CU(cudaMemcpyAsync(host_out, B.aos, n * elem, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
@@ -1889,27 +1848,21 @@ int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thres
   EF_LAUNCH(ctx, k_loop_constraints, 1, 256, 0, (const GNState*)ctx->odom[0].gn, (const GNState*)ctx->odom[1].gn, (const float4*)ctx->tex.vertex,
             (const uint16_t*)ctx->tex.old_time, m.rows, m.cols, ctx->max_depth_processed, count_thresh, err_thresh, cov_thresh, m.loop,
             m.loop_src, m.loop_dst, m.loop_times, m.loop_capacity);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 int map_loop_reset_async(EfContext* ctx) {
   EF_LAUNCH(ctx, k_loop_reset, 1, 32, 0, ctx->map.loop);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 int odom_copy_pose_async(EfContext* ctx, int dst, int src) {
   EF_LAUNCH(ctx, k_copy_pose, 1, 32, 0, ctx->odom[dst].gn, (const GNState*)ctx->odom[src].gn);
-  LAST();
+  CHECK_LAST();
   return 0;
 }
 
 // scan scratch shared with the tracker's per-frame candidate compaction (same stream, never concurrent)
-int scan_flags_shared(EfContext* ctx, const int* n_dev, size_t max_items, uint8_t** flags, int** offsets, int* total_dev) {
-  MapBuffers& B = mb(ctx);
-  *flags = ctx->map.flags;
-  *offsets = B.offsets;
-  return run_scan(ctx, ctx->map.flags, n_dev, nullptr, max_items, B.offsets, total_dev);
-}
 void scan_scratch(EfContext* ctx, uint8_t** flags, int** offsets) {
   *flags = ctx->map.flags;
   *offsets = mb(ctx).offsets;

@@ -72,14 +72,13 @@ int preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t
   const int rows = ctx->cfg.height, cols = ctx->cfg.width;
   dim3 grid((cols + TILE_X - 1) / TILE_X, (rows + TILE_Y - 1) / TILE_Y), block(TILE_X, TILE_Y);
   EF_LAUNCH(ctx, k_preprocess_depth, grid, block, 0, raw, rows, cols, cutoff, filtered, metric, metric_filtered);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : (int)e;
+  CHECK_LAST();
+  return 0;
 }
 int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba) {
   const size_t n = (size_t)ctx->cfg.height * ctx->cfg.width;
-  size_t b = (n + 255) / 256, cap = (size_t)ctx->num_sms * 8;
-  EF_LAUNCH(ctx, k_rgb_to_rgba, (int)(b < cap ? b : cap), 256, 0, rgb, (uchar4*)rgba, n);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : (int)e;
+  EF_LAUNCH(ctx, k_rgb_to_rgba, wave_blocks(ctx, n), 256, 0, rgb, (uchar4*)rgba, n);
+  CHECK_LAST();
+  return 0;
 }
 }  // namespace ef

@@ -464,31 +464,16 @@ __global__ void k_cand_scatter(SobelArgs a, const uint8_t* __restrict__ flags, c
 namespace {
 
 inline dim3 grid2d(int cols, int rows) { return dim3((cols + 31) / 32, (rows + 7) / 8); }
-inline int flat_blocks(const EfContext* ctx, size_t n) {
-  size_t b = (n + 255) / 256;
-  size_t cap = (size_t)ctx->num_sms * 8;
-  return (int)(b < cap ? (b ? b : 1) : cap);
-}
-
-#define EF_CHECK_LAST()                          \
-  do {                                           \
-    cudaError_t e__ = cudaGetLastError();        \
-    if (e__ != cudaSuccess) return (int)e__;     \
-  } while (0)
-
 }  // namespace
 
 namespace ef {
-int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_b, size_t max_items, int* offsets, int* total);
-void scan_scratch(EfContext* ctx, uint8_t** flags, int** offsets);
 
 int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff) {
   OdomDev& od = ctx->odom[which];
   ctx->maps_dirty[which] = true;
-  cudaError_t e = cudaMemcpyAsync(od.depth_tmp[0], depth_dev, sizeof(uint16_t) * od.width * od.height, cudaMemcpyDeviceToDevice, ctx->stream);
-  if (e != cudaSuccess) return (int)e;
+  CU(cudaMemcpyAsync(od.depth_tmp[0], depth_dev, sizeof(uint16_t) * od.width * od.height, cudaMemcpyDeviceToDevice, ctx->stream));
   for (int i = 1; i < NUM_PYRS; ++i)
-    EF_LAUNCH(ctx, k_pyr_down_u16, flat_blocks(ctx, (size_t)od.rows[i] * od.cols[i] * 2), 128, 0, od.depth_tmp[i - 1], od.rows[i - 1], od.cols[i - 1],
+    EF_LAUNCH(ctx, k_pyr_down_u16, wave_blocks(ctx, (size_t)od.rows[i] * od.cols[i] * 2), 128, 0, od.depth_tmp[i - 1], od.rows[i - 1], od.cols[i - 1],
               od.depth_tmp[i]);
   VmapArgs va;
   for (int i = 0; i < NUM_PYRS; ++i) {
@@ -506,19 +491,19 @@ int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, fl
     va.cy[i] = cy;
   }
   va.start[NUM_PYRS] = od.level_start[NUM_PYRS];
-  EF_LAUNCH(ctx, k_vmap_nmap, flat_blocks(ctx, (size_t)od.level_start[NUM_PYRS]), 256, 0, va, cutoff);
-  EF_CHECK_LAST();
+  EF_LAUNCH(ctx, k_vmap_nmap, wave_blocks(ctx, (size_t)od.level_start[NUM_PYRS]), 256, 0, va, cutoff);
+  CHECK_LAST();
   return 0;
 }
 
 static int copy_and_resize(EfContext* ctx, OdomDev& od, const float* vtx4, const float* nrm4, float** vm, float** nm) {
   const size_t n = (size_t)od.width * od.height;
-  EF_LAUNCH(ctx, k_copy_maps, flat_blocks(ctx, n), 256, 0, (const float4*)vtx4, (const float4*)nrm4, od.height, od.width, (float4*)od.vmaps_tmp,
+  EF_LAUNCH(ctx, k_copy_maps, wave_blocks(ctx, n), 256, 0, (const float4*)vtx4, (const float4*)nrm4, od.height, od.width, (float4*)od.vmaps_tmp,
             vm[0], nm[0]);
   const dim3 block(32, 8);
   for (int i = 1; i < NUM_PYRS; ++i)
     EF_LAUNCH(ctx, k_resize_maps, grid2d(od.cols[i], od.rows[i]), block, 0, vm[i - 1], nm[i - 1], od.rows[i - 1], od.cols[i - 1], vm[i], nm[i]);
-  EF_CHECK_LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -529,10 +514,9 @@ int odom_init_icp_pred(EfContext* ctx, int which, const float* vtx4, const float
 }
 
 // pose is taken from gn->T_wc (device) — callers that pass an explicit pose upload it first
-int odom_init_icp_model(EfContext* ctx, int which, const float* vtx4, const float* nrm4, bool with_global = true) {
+int odom_init_icp_model(EfContext* ctx, int which, const float* vtx4, const float* nrm4, bool with_global) {
   OdomDev& od = ctx->odom[which];
-  int rc = copy_and_resize(ctx, od, vtx4, nrm4, od.vmap_c_prev, od.nmap_c_prev);
-  if (rc) return rc;
+  RC(copy_and_resize(ctx, od, vtx4, nrm4, od.vmap_c_prev, od.nmap_c_prev));
   if (!with_global) return 0;  // the frame loop never reads the world-frame copy
   XformArgs a;
   for (int i = 0; i < NUM_PYRS; ++i) {
@@ -543,42 +527,42 @@ int odom_init_icp_model(EfContext* ctx, int which, const float* vtx4, const floa
     a.rows[i] = od.rows[i];
     a.cols[i] = od.cols[i];
   }
-  EF_LAUNCH(ctx, k_transform_maps, dim3(flat_blocks(ctx, (size_t)od.width * od.height), NUM_PYRS), 256, 0, a, (const GNState*)od.gn);
-  EF_CHECK_LAST();
+  EF_LAUNCH(ctx, k_transform_maps, dim3(wave_blocks(ctx, (size_t)od.width * od.height), NUM_PYRS), 256, 0, a, (const GNState*)od.gn);
+  CHECK_LAST();
   return 0;
 }
 
 // populateRGBDData (RGBDOdometry.cpp:212-234); with_depth=0 is initFirstRGB (:246-257)
 int odom_populate(EfContext* ctx, int which, const uint8_t* rgba, float** destDepths, uint8_t** destImages, bool with_depth,
-                  bool with_image = true) {
+                  bool with_image) {
   OdomDev& od = ctx->odom[which];
   const size_t n = (size_t)od.width * od.height;
-  EF_LAUNCH(ctx, k_depth_intensity_l0, flat_blocks(ctx, n), 256, 0, (const float4*)od.vmaps_tmp, (const uchar4*)rgba, n, od.maxDepthRGB,
+  EF_LAUNCH(ctx, k_depth_intensity_l0, wave_blocks(ctx, n), 256, 0, (const float4*)od.vmaps_tmp, (const uchar4*)rgba, n, od.maxDepthRGB,
             with_depth ? destDepths[0] : (float*)nullptr, with_image ? destImages[0] : (uint8_t*)nullptr);
   for (int i = 0; i + 1 < NUM_PYRS; ++i)
-    EF_LAUNCH(ctx, k_pyr_down_depth_image, flat_blocks(ctx, (size_t)od.rows[i + 1] * od.cols[i + 1] * 2), 128, 0,
+    EF_LAUNCH(ctx, k_pyr_down_depth_image, wave_blocks(ctx, (size_t)od.rows[i + 1] * od.cols[i + 1] * 2), 128, 0,
               with_depth ? destDepths[i] : (const float*)nullptr, with_depth ? destDepths[i + 1] : (float*)nullptr,
               with_image ? (const uint8_t*)destImages[i] : (const uint8_t*)nullptr, with_image ? destImages[i + 1] : (uint8_t*)nullptr, od.rows[i],
               od.cols[i]);
-  EF_CHECK_LAST();
+  CHECK_LAST();
   return 0;
 }
 
 // frameToModel.initICPModel + initRGBModel with the reference's fill-in choice (ElasticFusion.cpp:302-315) resolved on
 // the device: predicted maps when the model view is dense enough, FillIn maps otherwise.
-int map_select_model_inputs(EfContext* ctx, const float**, const float**, const uint8_t**) {
+int map_select_model_inputs(EfContext* ctx) {
   OdomDev& od = ctx->odom[0];
   Textures& t = ctx->tex;
   const size_t n = (size_t)od.width * od.height;
-  EF_LAUNCH(ctx, k_model_level0, flat_blocks(ctx, n), 256, 0, (const float4*)t.vertex, (const float4*)t.normal, (const float4*)t.fill_vertex,
+  EF_LAUNCH(ctx, k_model_level0, wave_blocks(ctx, n), 256, 0, (const float4*)t.vertex, (const float4*)t.normal, (const float4*)t.fill_vertex,
             (const float4*)t.fill_normal, (const uchar4*)t.image, (const uchar4*)t.fill_image, (const int*)ctx->map.dense_flag,
             ctx->frame_to_frame_rgb ? 1 : 0, od.height, od.width, od.maxDepthRGB, (float4*)od.vmaps_tmp, od.vmap_c_prev[0], od.nmap_c_prev[0],
             od.lastDepth[0], od.lastImage[0]);
   for (int i = 0; i + 1 < NUM_PYRS; ++i)
-    EF_LAUNCH(ctx, k_model_level_down, flat_blocks(ctx, (size_t)od.rows[i + 1] * od.cols[i + 1] * 2), 128, 0, (const float*)od.vmap_c_prev[i],
+    EF_LAUNCH(ctx, k_model_level_down, wave_blocks(ctx, (size_t)od.rows[i + 1] * od.cols[i + 1] * 2), 128, 0, (const float*)od.vmap_c_prev[i],
               (const float*)od.nmap_c_prev[i], (const float*)od.lastDepth[i], (const uint8_t*)od.lastImage[i], od.rows[i], od.cols[i],
               od.vmap_c_prev[i + 1], od.nmap_c_prev[i + 1], od.lastDepth[i + 1], od.lastImage[i + 1]);
-  EF_CHECK_LAST();
+  CHECK_LAST();
   return 0;
 }
 
@@ -600,12 +584,11 @@ int launch_sobel(EfContext* ctx, int which) {
   uint8_t* flags;
   int* offsets;
   scan_scratch(ctx, &flags, &offsets);
-  EF_LAUNCH(ctx, k_sobel_cand, flat_blocks(ctx, flat), 256, 0, a, flags);
-  int rc = run_scan(ctx, flags, &od.gn->flat_n, nullptr, flat, offsets, &od.gn->cand_base[NUM_PYRS]);
-  if (rc) return rc;
-  EF_LAUNCH(ctx, k_cand_scatter, flat_blocks(ctx, flat), 256, 0, a, (const uint8_t*)flags, (const int*)offsets, od.cand, od.gn);
+  EF_LAUNCH(ctx, k_sobel_cand, wave_blocks(ctx, flat), 256, 0, a, flags);
+  RC(run_scan(ctx, flags, &od.gn->flat_n, nullptr, flat, offsets, &od.gn->cand_base[NUM_PYRS]));
+  EF_LAUNCH(ctx, k_cand_scatter, wave_blocks(ctx, flat), 256, 0, a, (const uint8_t*)flags, (const int*)offsets, od.cand, od.gn);
   ctx->maps_dirty[which] = true;  // k_iter1 / k_iter2 read the list ahead of their dependency wait: fence before the next one
-  EF_CHECK_LAST();
+  CHECK_LAST();
   return 0;
 }
 
