@@ -39,6 +39,11 @@ class EfDeformResult(C.Structure):
                 ("stop", C.c_int32), ("bandwidth", C.c_int32), ("error", C.c_float), ("meanConsErr", C.c_float)]
 
 
+class EfLocalDeform(C.Structure):
+    _fields_ = [("solved", C.c_int32), ("applied", C.c_int32), ("result", EfDeformResult), ("deforms", C.c_int32),
+                ("last_deform_time", C.c_int32), ("n_nodes", C.c_int32)]
+
+
 TRACE_DTYPE = np.dtype([
     ("kind", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("rgb_count", "<i4"), ("rgb_sigma", "<i4"),
     ("sigma_val", "<f4"),
@@ -251,6 +256,17 @@ class Context:
         info = {k: getattr(res, k) for k, _ in EfDeformResult._fields_}
         R = rt[:n, :9].reshape(n, 3, 3).transpose(0, 2, 1).copy()  # column-major -> R[i, row, col]
         return info, nodes[:n], cn[:m], cw[:m], R, rt[:n, 9:].copy()
+
+    def local_deform_result(self):
+        """close_loops = 2: (info dict, graph (n, 4) float32: x y z time per node) of the last frame's in-frame loop closure.
+        info: solved, applied, result (EfDeformResult fields, all zero unless solved), deforms, last_deform_time, n_nodes."""
+        res = EfLocalDeform()
+        nodes = np.zeros((1023, 4), np.float32)
+        n = C.c_int32()
+        _chk(lib().ef_local_deform_result(self.h_ctx, C.byref(res), _p(nodes), len(nodes), C.byref(n)))
+        info = dict(solved=bool(res.solved), applied=bool(res.applied), result={k: getattr(res.result, k) for k, _ in EfDeformResult._fields_},
+                    deforms=res.deforms, last_deform_time=res.last_deform_time, n_nodes=res.n_nodes)
+        return info, nodes[:n.value].copy()
 
     def predict(self):
         _chk(lib().ef_predict(self.h_ctx))

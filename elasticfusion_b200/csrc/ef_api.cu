@@ -219,7 +219,9 @@ static int create_buffers(EfContext* ctx) {
 extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
   if (!cfg || !out || cfg->width <= 0 || cfg->height <= 0 || cfg->capacity <= 0) return EF_EINVAL;
   // close_loops = 1 runs the LOCAL loop closure front half every frame (ElasticFusion.cpp:447-505; results through
-  // ef_local_loop_result). Ferns / relocalisation and the deformation solve stay outside this library (SURVEY.md §8).
+  // ef_local_loop_result); 2 also samples, solves and applies the deformation graph inside the frame (frame_local_deform).
+  // Ferns / relocalisation stay outside this library (SURVEY.md §8).
+  if (cfg->close_loops < 0 || cfg->close_loops > 2) return EF_EINVAL;
   if (cfg->reloc) return EF_EINVAL;
   if ((cfg->width >> 2) < 8 || (cfg->height >> 2) < 8) return EF_EINVAL;
   CU(cudaSetDevice(cfg->device));
@@ -955,11 +957,53 @@ static int frame_end_device(EfContext* ctx, int n_nodes, bool fern_accepted) {
   return 0;
 }
 
+// close_loops = 2: the rest of a frame whose first half frame_begin_device has enqueued, with the local loop closure closed inside it
+// (ElasticFusion.cpp:505-534, 536-593; no fern matched). When the front half ran, one small record is read back: whether it
+// accepted, its constraint count and the node count of the graph sampled at the end of the previous frame. A graph exists once
+// some frame sampled more than 4 nodes (Deformation::def.isInit()). On an accepted closure with a graph and at least one
+// constraint, the graph is solved on the device (pinned while nothing has been deformed, nodes up to lastDeformTime fixed)
+// and the solve's result is read back. Its nodes go to the clean and T_wc_est becomes the pose, whatever the solve's stop rule
+// (the reference applies the graph unconditionally without a fern match), except stop 6, where nothing was solved. Then the
+// second half of the frame and, after clean as at :593, the graph for the next frame is sampled.
+static int frame_local_deform(EfContext* ctx) {
+  ctx->deform_solved = ctx->deform_applied = false;
+  memset(&ctx->deform_result, 0, sizeof(ctx->deform_result));
+  int n_nodes = 0;
+  if (ctx->tick > 1 && !ctx->rgb_only) {  // the front half ran (frame_begin_device)
+    MapDev& m = ctx->map;
+    PinStaging* s = ctx->pin_small;
+    CU(cudaMemcpyAsync(s->loop_record, &m.loop->accepted, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(s->loop_record + 2, m.graph_n, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const int accepted = s->loop_record[0], n_cons = s->loop_record[1], graph_n = s->loop_record[2];
+    if (accepted && graph_n > 0 && n_cons > 0) {
+      const float* nodes16 = nullptr;
+      RC(deform_solve_local(ctx, m.graph, graph_n, m.loop_src, m.loop_dst, m.loop_times, n_cons, ctx->deforms == 0, ctx->tick,
+                            ctx->last_deform_time, &s->deform_result, &nodes16));
+      ctx->deform_solved = true;
+      ctx->deform_result = s->deform_result;
+      if (ctx->deform_result.stop != 6) {
+        // ef_process_frame_end(T_wc_est, graph): the pose, the map kernels' copy of it and the nodes the clean reads
+        CU(cudaMemcpyAsync(ctx->odom[0].gn->T_wc, m.loop->T_wc_est, sizeof(double) * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+        RC(map_update_pose_async(ctx, nullptr));
+        RC(map_set_graph_device(ctx, nodes16, graph_n));
+        n_nodes = graph_n;
+        ctx->deform_applied = true;
+        ctx->deforms += 1;                   // ElasticFusion.cpp:518
+        ctx->last_deform_time = ctx->tick;   // Deformation.cpp:191-193
+      }
+    }
+  }
+  RC(frame_end_device(ctx, n_nodes, false));
+  return map_sample_graph_async(ctx);  // (predict, which frame_end_device ran after clean, leaves the surfels as they are)
+}
+
 extern "C" int ef_process_frame_device(EfContext* ctx, const uint8_t* rgb_dev, const uint16_t* depth_dev, int64_t timestamp,
                                        float weight_multiplier, const double* in_T_wc) {
   (void)timestamp;
   if (!ctx || ((rgb_dev == nullptr) != (depth_dev == nullptr))) return EF_EINVAL;
   RC(frame_begin_device(ctx, rgb_dev, depth_dev, weight_multiplier, in_T_wc));
+  if (ctx->cfg.close_loops == 2) return frame_local_deform(ctx);
   return frame_end_device(ctx, 0, false);
 }
 
@@ -982,7 +1026,7 @@ extern "C" int ef_process_frame_begin(EfContext* ctx, const uint8_t* rgb, const 
                                       const double* in_T_wc) {
   (void)timestamp;
   if (!ctx || !rgb || !depth) return EF_EINVAL;
-  if (ctx->la.pending || ctx->frame_open) return EF_ESTATE;
+  if (ctx->la.pending || ctx->frame_open || ctx->cfg.close_loops == 2) return EF_ESTATE;  // mode 2 closes its loops itself
   RC(stage_host_frame(ctx, rgb, depth));
   RC(frame_begin_device(ctx, ctx->tex.rgb, ctx->tex.depth_raw, weight_multiplier, in_T_wc));
   return ef_finish_frame(ctx);  // pose (and the loop-closure result) are final on return
@@ -990,7 +1034,7 @@ extern "C" int ef_process_frame_begin(EfContext* ctx, const uint8_t* rgb, const 
 
 extern "C" int ef_process_frame_end(EfContext* ctx, const double* T_wc_override, const float* graph_nodes16, int32_t n_nodes, int32_t fern_accepted) {
   if (!ctx || n_nodes < 0 || (n_nodes > 0 && !graph_nodes16)) return EF_EINVAL;
-  if (!ctx->frame_open) return EF_ESTATE;
+  if (!ctx->frame_open || ctx->cfg.close_loops == 2) return EF_ESTATE;
   if (T_wc_override) {
     RC(ef_set_pose(ctx, T_wc_override));
     RC(map_update_pose_async(ctx, nullptr));
@@ -998,6 +1042,26 @@ extern "C" int ef_process_frame_end(EfContext* ctx, const double* T_wc_override,
   RC(map_set_graph(ctx, graph_nodes16, n_nodes));
   RC(frame_end_device(ctx, n_nodes, fern_accepted != 0));
   return ef_finish_frame(ctx);
+}
+
+extern "C" int ef_local_deform_result(EfContext* ctx, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out) {
+  if (!ctx || !out || max_nodes < 0 || (max_nodes > 0 && !nodes4)) return EF_EINVAL;
+  if (ctx->cfg.close_loops != 2) return EF_ESTATE;
+  int n = 0;
+  RC(read_count(ctx, ctx->map.graph_n, &n));
+  out->solved = ctx->deform_solved;
+  out->applied = ctx->deform_applied;
+  out->result = ctx->deform_result;
+  out->deforms = ctx->deforms;
+  out->last_deform_time = ctx->last_deform_time;
+  out->n_nodes = n;
+  if (n > max_nodes) n = max_nodes;
+  if (n_out) *n_out = n;
+  if (n > 0) {
+    CU(cudaMemcpyAsync(nodes4, ctx->map.graph, sizeof(float) * 4 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
 }
 
 extern "C" int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* src3, double* dst3, int32_t* times, int32_t max_constraints,

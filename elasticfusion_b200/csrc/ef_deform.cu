@@ -611,19 +611,13 @@ void deform_free(EfContext* ctx) {
   ctx->deform = nullptr;
 }
 
-// Device-side inputs are uploaded from `host` (pinned by the caller or pageable); the solve itself is one launch.
-int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
-                 const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
-                 int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out) {
+static DeformWork* work(EfContext* ctx) {
   if (!ctx->deform) ctx->deform = new DeformWork();
-  DeformWork* w = static_cast<DeformWork*>(ctx->deform);
-  RC(reserve(w, n, m));
-  cudaStream_t st = ctx->stream;
-  CU(cudaMemcpyAsync(w->pos, node_pos3, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(w->ntime, node_times, sizeof(int) * n, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(w->src, src3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(w->dst, dst3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(w->ctime, src_times, sizeof(int) * m, cudaMemcpyHostToDevice, st));
+  return static_cast<DeformWork*>(ctx->deform);
+}
+
+// the one solve launch: n nodes (pos, ntime) and m constraints (src, dst, ctime) already in the workspace
+static int launch_solve(EfContext* ctx, DeformWork* w, int n, int m, int last_deform_time) {
   Args a;
   a.n = n;
   a.m = m;
@@ -641,12 +635,75 @@ int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_ti
   a.out = w->out;
   EF_LAUNCH(ctx, k_deform_solve, 1, THREADS, 0, a);
   CHECK_LAST();
+  return 0;
+}
+
+// Device-side inputs are uploaded from `host` (pinned by the caller or pageable); the solve itself is one launch.
+int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
+                 const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
+                 int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out) {
+  DeformWork* w = work(ctx);
+  RC(reserve(w, n, m));
+  cudaStream_t st = ctx->stream;
+  CU(cudaMemcpyAsync(w->pos, node_pos3, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->ntime, node_times, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->src, src3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->dst, dst3, sizeof(double) * 3 * m, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(w->ctime, src_times, sizeof(int) * m, cudaMemcpyHostToDevice, st));
+  RC(launch_solve(ctx, w, n, m, last_deform_time));
   CU(cudaMemcpyAsync(out, w->out, sizeof(EfDeformResult), cudaMemcpyDeviceToHost, st));
   if (nodes16_host) CU(cudaMemcpyAsync(nodes16_host, w->nodes16, sizeof(float) * 16 * n, cudaMemcpyDeviceToHost, st));
   if (rt12_host) CU(cudaMemcpyAsync(rt12_host, w->rt12, sizeof(double) * 12 * n, cudaMemcpyDeviceToHost, st));
   if (cons_nodes4) CU(cudaMemcpyAsync(cons_nodes4, w->cnode, sizeof(int) * KNN * m, cudaMemcpyDeviceToHost, st));
   if (cons_weights4) CU(cudaMemcpyAsync(cons_weights4, w->cw, sizeof(double) * KNN * m, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// Solve inputs of an in-frame local closure, what Deformation::sampleGraphFrom / addConstraint / constrain hand the graph
+// (Deformation.cpp:73-86, 119-132, 306-330): node positions widened to fp64 and times truncated to integers; constraint i is
+// (src, dst) at time src_time, followed by its pin (dst, dst) at dst_times[i] when `pin` is set.
+__global__ void k_deform_inputs(const float4* __restrict__ graph, int n, const double* __restrict__ src3, const double* __restrict__ dst3,
+                                const int* __restrict__ dst_times, int n_cons, int pin, int src_time, double* __restrict__ pos,
+                                int* __restrict__ ntime, double* __restrict__ src, double* __restrict__ dst, int* __restrict__ ctime) {
+  pdl_enter();
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(n, n_cons); i += gridDim.x * blockDim.x) {
+    if (i < n) {
+      const float4 g = graph[i];
+      pos[3 * i] = g.x;
+      pos[3 * i + 1] = g.y;
+      pos[3 * i + 2] = g.z;
+      ntime[i] = (int)g.w;
+    }
+    if (i < n_cons) {
+      const int o = pin ? 2 * i : i;
+      for (int q = 0; q < 3; ++q) {
+        src[3 * o + q] = src3[3 * i + q];
+        dst[3 * o + q] = dst3[3 * i + q];
+      }
+      ctime[o] = src_time;
+      if (pin) {
+        for (int q = 0; q < 3; ++q) src[3 * (o + 1) + q] = dst[3 * (o + 1) + q] = dst3[3 * i + q];
+        ctime[o + 1] = dst_times[i];
+      }
+    }
+  }
+}
+
+// Deformation::constrain of a local closure inside the frame: inputs gathered on the device, the same solve as deform_solve,
+// then the solve's result read back into `out` (pinned). *nodes16_dev: the hand-over, valid until the next solve.
+int deform_solve_local(EfContext* ctx, const float4* graph, int n, const double* src3, const double* dst3, const int* dst_times, int n_cons,
+                       bool pin, int src_time, int last_deform_time, EfDeformResult* out, const float** nodes16_dev) {
+  DeformWork* w = work(ctx);
+  const int m = pin ? 2 * n_cons : n_cons;
+  RC(reserve(w, n, m));
+  EF_LAUNCH(ctx, k_deform_inputs, 4, 256, 0, graph, n, src3, dst3, dst_times, n_cons, pin ? 1 : 0, src_time, w->pos, w->ntime, w->src, w->dst,
+            w->ctime);
+  CHECK_LAST();
+  RC(launch_solve(ctx, w, n, m, last_deform_time));
+  CU(cudaMemcpyAsync(out, w->out, sizeof(EfDeformResult), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  *nodes16_dev = w->nodes16;
   return 0;
 }
 

@@ -166,6 +166,10 @@ struct MapDev {
   int loop_capacity;      // loop_constraint_capacity(cols, rows)
   double *loop_src, *loop_dst;  // loop_capacity x 3: vert_w_curr / vert_w_est of each constraint
   int* loop_times;              // loop_capacity: the INACTIVE view's time stamp of each constraint
+  // close_loops = 2 only: the deformation graph sampled at the end of the last frame (Deformation::rawSampledNodes_w: xyz and
+  // init time of every 5000th surfel, at most MAX_GRAPH_NODES - 1) and its node count (0 until a frame sampled more than 4)
+  float4* graph;
+  int* graph_n;
 };
 
 struct Textures {
@@ -239,6 +243,8 @@ struct PinStaging {
   double T_wc[16];       // frame_begin_device: the caller's pose for a frame that is not tracked
   double finish_T_wc[16];  // ef_finish_frame: pose and surfel count read back
   int finish_count;
+  int loop_record[3];              // close_loops = 2, mid-frame: LoopDev::accepted, LoopDev::n_constraints, MapDev::graph_n
+  EfDeformResult deform_result;    // close_loops = 2: the frame's deformation solve
 };
 // Layout of the device staging block (EfContext::dev_small): where the kernels read the pinned slots above.
 struct DevStaging {
@@ -283,6 +289,10 @@ struct EfContext {
   float confidence, depth_cutoff, max_depth_processed;
   int host_count;  // last count read back
   bool frame_open; // ef_process_frame_begin has run, ef_process_frame_end has not
+  // close_loops = 2: Deformation's bookkeeping (ElasticFusion::deforms, Deformation::lastDeformTime) and the last frame's outcome
+  int deforms, last_deform_time;
+  bool deform_solved, deform_applied;
+  EfDeformResult deform_result;
 
   // pinned staging
   uint8_t* pin_rgb;
@@ -404,6 +414,8 @@ int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, 
 int map_fuse_async(EfContext* ctx, int time_or_neg, float max_depth, float weighting_or_neg);
 int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0, bool is_fern = false);
 int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);
+int map_set_graph_device(EfContext* ctx, const float* nodes16_dev, int n_nodes);
+int map_sample_graph_async(EfContext* ctx);
 int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode);
 int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
 int map_dense_enough_async(EfContext* ctx);
@@ -419,5 +431,7 @@ int map_resize_to_host(EfContext* ctx, const void* src_dev, int elem, int factor
 int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,
                  const int32_t* src_times, int m, int last_deform_time, float* nodes16_host, double* rt12_host,
                  int32_t* cons_nodes4, double* cons_weights4, EfDeformResult* out);
+int deform_solve_local(EfContext* ctx, const float4* graph, int n, const double* src3, const double* dst3, const int* dst_times, int n_cons,
+                       bool pin, int src_time, int last_deform_time, EfDeformResult* out, const float** nodes16_dev);
 void deform_free(EfContext* ctx);
 }  // namespace ef

@@ -1469,6 +1469,10 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &m.loop_src, (size_t)m.loop_capacity * 3));
   CU(ctx_alloc(ctx, &m.loop_dst, (size_t)m.loop_capacity * 3));
   CU(ctx_alloc(ctx, &m.loop_times, (size_t)m.loop_capacity));
+  if (c.close_loops == 2) {
+    CU(ctx_alloc(ctx, &m.graph, (size_t)MAX_GRAPH_NODES - 1, 0));
+    CU(ctx_alloc(ctx, &m.graph_n, 1, 0));
+  }
   B->scan_epoch = 0;
   B->scan_state_bytes = tiles * 8;
   const int one = 1;
@@ -1752,6 +1756,37 @@ int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes) {
   CU(cudaStreamSynchronize(ctx->stream));
   CU(cudaMemcpyAsync(m.nodes, nodes16, (size_t)n_nodes * 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));  // nodes16 is caller memory
+  return 0;
+}
+// the same from a device buffer (the device solve's hand-over), stream-ordered
+int map_set_graph_device(EfContext* ctx, const float* nodes16_dev, int n_nodes) {
+  if (n_nodes < 0 || n_nodes >= MAX_GRAPH_NODES) return EF_EINVAL;
+  if (n_nodes > 0)
+    CU(cudaMemcpyAsync(ctx->map.nodes, nodes16_dev, (size_t)n_nodes * 16 * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+  return 0;
+}
+
+// Deformation::sampleGraphModel (Deformation.cpp:248-303, sample.geom): position and colorTime.z (init time) of surfels 0, 5000,
+// 10000, ... The graph is replaced only when more than k = 4 nodes come out (:284); otherwise the previous one stays. The
+// reference's transform-feedback buffer holds 1024 nodes and keeps the oldest ones (Deformation.cpp:27); here the cap is 1023,
+// the largest graph clean accepts (GlobalModel.cpp:540 asserts fewer than MAX_NODES = 1024), so maps of more than 5 110 000
+// surfels sample one node fewer than the reference does.
+__global__ void k_sample_graph(const float4* __restrict__ pos_conf, const float4* __restrict__ color_time, const int* __restrict__ count,
+                               float4* __restrict__ graph, int* __restrict__ graph_n) {
+  pdl_enter();
+  const int sampled = (*count + 4999) / 5000;
+  if (sampled <= 4) return;
+  const int n = min(sampled, MAX_GRAPH_NODES - 1);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float4 p = pos_conf[(size_t)i * 5000];
+    graph[i] = make_float4(p.x, p.y, p.z, color_time[(size_t)i * 5000].z);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *graph_n = n;
+}
+int map_sample_graph_async(EfContext* ctx) {
+  MapDev& m = ctx->map;
+  EF_LAUNCH(ctx, k_sample_graph, 4, 256, 0, (const float4*)m.pos_conf, (const float4*)m.color_time, (const int*)m.count, m.graph, m.graph_n);
+  CHECK_LAST();
   return 0;
 }
 

@@ -10,7 +10,9 @@
 //
 // (reference README.md:74-100, MainController.cpp:178-243) compiles and runs unchanged, minus OpenGL display: there is
 // no GL context to create, GPUTexture wraps a CUDA device buffer, and model() returns an opaque handle.
-// Loop closure (closeLoops / reloc, Ferns, Deformation) is outside this library's scope: the constructor refuses it.
+// Relocalisation and global (fern) loop closures are outside this library's scope: the constructor refuses reloc. Local loop
+// closures: closeLoops runs the front half on the device; with the trailing deviceLoopClosure = true processFrame also
+// samples, solves and applies the deformation graph (ef_create with close_loops = 2).
 //
 // If <sophus/se3.hpp> is on the include path the pose types are Sophus::SE3d exactly as in the reference; otherwise a
 // minimal ef::SE3d with the members the reference API uses (matrix(), translation(), rotationMatrix(), inverse()).
@@ -295,19 +297,20 @@ class ElasticFusion {
                 const bool closeLoops = true, const bool iclnuim = false, const bool reloc = false, const float photoThresh = 115,
                 const float confidence = 10, const float depthCut = 3, const float icpThresh = 10, const bool fastOdom = false,
                 const float fernThresh = 0.3095, const bool so3 = true, const bool frameToFrameRGB = false, const std::string fileName = "",
-                const int surfelCapacity = 3072 * 3072, const int device = 0)
-      : saveFilename(fileName), iclnuim_(iclnuim), confidenceThreshold_(confidence), maxDepthProcessed_(20.0f), timeDelta_(timeDelta) {
+                const int surfelCapacity = 3072 * 3072, const int device = 0, const bool deviceLoopClosure = false)
+      : saveFilename(fileName), iclnuim_(iclnuim), confidenceThreshold_(confidence), maxDepthProcessed_(20.0f), timeDelta_(timeDelta),
+        deviceLoopClosure_(closeLoops && deviceLoopClosure) {
     if (reloc) {
       std::fprintf(stderr,
                    "ElasticFusion(b200): relocalisation (Ferns) is outside this library's scope; construct with reloc=false.\n");
       std::exit(1);
     }
-    if (closeLoops)
+    if (closeLoops && !deviceLoopClosure_)
       std::fprintf(stderr,
                    "ElasticFusion(b200): closeLoops=true runs the LOCAL loop closure front half on the device every frame (registration of "
                    "the active against the inactive model view, acceptance test, constraint sampling: getLocalLoopClosure()); the "
                    "deformation solve (Deformation::constrain) and Ferns are not part of this library, so the map stays open-loop unless "
-                   "the caller feeds processFrameEnd() a graph.\n");
+                   "the caller feeds processFrameEnd() a graph, or deviceLoopClosure=true lets processFrame() close local loops itself.\n");
     EfConfig cfg;
     ef_default_config(&cfg, Resolution::getInstance().width(), Resolution::getInstance().height(), Intrinsics::getInstance().fx(),
                       Intrinsics::getInstance().fy(), Intrinsics::getInstance().cx(), Intrinsics::getInstance().cy());
@@ -315,7 +318,7 @@ class ElasticFusion {
     cfg.count_thresh = countThresh;
     cfg.err_thresh = errThresh;
     cfg.cov_thresh = covThresh;
-    cfg.close_loops = closeLoops ? 1 : 0;
+    cfg.close_loops = deviceLoopClosure_ ? 2 : closeLoops ? 1 : 0;  // 2: sample, solve and apply the deformation graph in the frame
     cfg.iclnuim = iclnuim;
     cfg.photo_thresh = photoThresh;
     cfg.confidence = confidence;
@@ -466,7 +469,15 @@ class ElasticFusion {
   void setTick(const int& val) { ef::check(ef_set_tick(ctx_, val), "setTick"); }
   const float& getMaxDepthProcessed() { return maxDepthProcessed_; }
   const ef::SE3d& get_T_wc() { return T_wc_curr_; }
-  const int& getDeforms() { return zero_; }
+  // local loop closures applied so far; they happen inside processFrame only with deviceLoopClosure
+  const int& getDeforms() {
+    if (deviceLoopClosure_) {
+      EfLocalDeform d;
+      ef::check(ef_local_deform_result(ctx_, &d, nullptr, 0, nullptr), "getDeforms");
+      deforms_ = d.deforms;
+    }
+    return deforms_;
+  }
   const int& getFernDeforms() { return zero_; }
 
   // binary little-endian PLY, x y z r g b nx ny nz radius, normals negated, only surfels above the confidence threshold
@@ -552,6 +563,8 @@ class ElasticFusion {
   int timeDelta_;
   int tick_ = 1;
   int zero_ = 0;
+  int deforms_ = 0;
+  const bool deviceLoopClosure_;  // close_loops = 2
   bool lost_ = false;
   bool staged_ = false;  // a look-ahead frame is waiting in the library (ef_prefetch_frame)
   int64_t pendingTimestamp_ = 0;

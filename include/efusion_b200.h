@@ -41,8 +41,10 @@ typedef struct {
   int32_t count_thresh;   /* 35000  (loop closure only; kept for API parity) */
   float err_thresh;       /* 5e-05  (loop closure only) */
   float cov_thresh;       /* 1e-05  (loop closure only) */
-  int32_t close_loops;    /* 1: run the local loop closure front half every frame (results: ef_local_loop_result); the
-                             deformation solve and Ferns stay with the host (SURVEY.md §8) */
+  int32_t close_loops;    /* 0: open loop. 1: run the local loop closure front half every frame (results: ef_local_loop_result);
+                             the deformation solve stays with the host (ef_process_frame_begin / _end). 2: close local loops
+                             inside the frame as well -- sample, solve and apply the deformation graph (ef_local_deform_result).
+                             Other values: EF_EINVAL. Ferns stay outside this library (SURVEY.md §8) */
   int32_t iclnuim;
   int32_t reloc;          /* must be 0 */
   float photo_thresh;     /* 115 (ferns only) */
@@ -72,7 +74,9 @@ const char* ef_error_string(int code);
  * in_T_wc may be NULL (track) or a pose to use instead of tracking. Returns after get_T_wc-observable state is final. */
 int ef_process_frame(EfContext* ctx, const uint8_t* rgb, const uint16_t* depth, int64_t timestamp,
                      float weight_multiplier, const double* in_T_wc);
-/* same with inputs already resident in HBM; fully asynchronous (no host sync) — call ef_sync before reading results */
+/* same with inputs already resident in HBM; fully asynchronous (no host sync) — call ef_sync before reading results. Except
+ * with cfg.close_loops = 2: then the host reads a 12-byte record once the loop closure front half has run, and on a frame that
+ * solves a deformation graph it also waits for the solve (see ef_local_deform_result) */
 int ef_process_frame_device(EfContext* ctx, const uint8_t* rgb_dev, const uint16_t* depth_dev, int64_t timestamp,
                             float weight_multiplier, const double* in_T_wc);
 int ef_sync(EfContext* ctx);
@@ -98,7 +102,8 @@ int ef_finish_frame(EfContext* ctx);
  * results are final on return. ef_process_frame_end: optional pose override (T_wc_curr = T_wc_est, :524) and deformation graph
  * (16 floats per node: position 3, rotation 9 column-major, translation 3, time -- Core/Deformation.cpp:175-189) applied inside
  * clean (Core/Shaders/copy_unstable.vert:132-322), then index map / fuse / index map / clean / predict, tick++.
- * ef_process_frame == begin + end(NULL, NULL, 0, 0). EF_ESTATE if the calls are not paired. */
+ * ef_process_frame == begin + end(NULL, NULL, 0, 0). EF_ESTATE if the calls are not paired, and with cfg.close_loops = 2, which
+ * runs the solve inside ef_process_frame. */
 int ef_process_frame_begin(EfContext* ctx, const uint8_t* rgb, const uint16_t* depth, int64_t timestamp, float weight_multiplier,
                            const double* in_T_wc);
 int ef_process_frame_end(EfContext* ctx, const double* T_wc_override, const float* graph_nodes16, int32_t n_nodes,
@@ -141,6 +146,24 @@ int ef_deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node
                     const double* dst3, const int32_t* src_times, const int32_t* dst_times, int32_t n_constraints, int32_t pin,
                     int32_t last_deform_time, float* nodes16, double* rt12, int32_t* cons_nodes4, double* cons_weights4,
                     EfDeformResult* out);
+/* cfg.close_loops = 2: the local loop closure closed inside ef_process_frame / ef_process_frame_device (Core/ElasticFusion.cpp:
+ * 447-534 and 593 without ferns, Core/Deformation.cpp). After each frame the graph is sampled from the map: position and init time
+ * of surfels 0, 5000, 10000, ... (sample.geom), at most 1023 nodes (the reference keeps 1024: maps of more than 5 110 000 surfels
+ * get one node fewer), kept from the previous frame when 4 or fewer come out. When the front half of a later frame accepts, has at
+ * least one constraint and a graph exists, the graph is solved as ef_deform_solve solves it (pin = (deforms == 0), constraint
+ * source time = the frame's tick, last_deform_time) and, unless the solve stopped with code 6, applied: T_wc = T_wc_est and the
+ * nodes go to the frame's clean, as ef_process_frame_end(T_wc_est, nodes) does; then deforms += 1, last_deform_time = tick. */
+typedef struct {
+  int32_t solved;            /* the last frame ran the solve */
+  int32_t applied;           /* ... and applied its graph and pose */
+  EfDeformResult result;     /* that solve's result; all zero when !solved */
+  int32_t deforms;           /* closures applied since ef_create (ElasticFusion::getDeforms) */
+  int32_t last_deform_time;  /* tick of the last applied closure (Deformation::lastDeformTime); 0 before the first */
+  int32_t n_nodes;           /* nodes of the current graph (0: none sampled yet) */
+} EfLocalDeform;
+/* nodes4 (HOST, may be NULL when max_nodes = 0): the current graph, x y z and time per node (Deformation::rawSampledNodes_w);
+ * n_out: how many were written. EF_ESTATE unless cfg.close_loops = 2. */
+int ef_local_deform_result(EfContext* ctx, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out);
 /* ElasticFusion::predict (Core/ElasticFusion.cpp:621-653) */
 int ef_predict(EfContext* ctx);
 

@@ -7,7 +7,8 @@
 //   -p <poses>   ground-truth poses to use instead of tracking   -c -d -i -ie -cv -pt -ft -t -ic -s -e   as the reference
 //   -icl  -o  -rl(refused)  -fs  -q(implied)  -fo  -nso  -f  -ftf  -r(ignored: nothing to watch)
 // additions: -w <width> -h <height> (default 640 480), -cap <surfels>, -dev <cuda device>, -ply (write the map at the end),
-//            -nola (no frame look-ahead), -v (per-frame line)
+//            -nola (no frame look-ahead), -v (per-frame line), -dlc (without -o: close local loops inside processFrame, i.e.
+//            sample, solve and apply the deformation graph on the device; prints the number of closures applied)
 #include <ElasticFusion.h>
 #include <Tools/RawLogReader.h>
 
@@ -111,7 +112,7 @@ int main(int argc, char** argv) {
   getArg(argc, argv, "-l", logFile);
   if (logFile.empty() || findArg(argc, argv, "--help") > 0) {
     std::fprintf(stderr, "usage: %s -l <log.klg> [-cal <file>] [-w W -h H] [-o] [-icl] [-fo] [-nso] [-f] [-ftf] [-c conf] [-d depth] [-i icp] "
-                         "[-t timeDelta] [-s start] [-e end] [-p poses] [-cap surfels] [-dev n] [-ply] [-nola] [-v]\n", argv[0]);
+                         "[-t timeDelta] [-s start] [-e end] [-p poses] [-cap surfels] [-dev n] [-ply] [-nola] [-v] [-dlc]\n", argv[0]);
     return 2;
   }
   int width = 640, height = 480;
@@ -159,10 +160,12 @@ int main(int argc, char** argv) {
   const bool reloc = findArg(argc, argv, "-rl") > 0, frameskip = findArg(argc, argv, "-fs") > 0, fastOdom = findArg(argc, argv, "-fo") > 0;
   const bool so3 = !(findArg(argc, argv, "-nso") > 0), frameToFrameRGB = findArg(argc, argv, "-ftf") > 0;
   const bool lookahead = !(findArg(argc, argv, "-nola") > 0) && !frameskip, verbose = findArg(argc, argv, "-v") > 0;
+  const bool deviceLoopClosure = !openLoop && findArg(argc, argv, "-dlc") > 0;
 
   RawLogReader reader(logFile, flip);
   ElasticFusion eFusion(openLoop ? std::numeric_limits<int>::max() / 2 : timeDelta, icpCountThresh, icpErrThresh, covThresh, !openLoop, iclnuim, reloc,
-                        photoThresh, confidence, depth, icp, fastOdom, fernThresh, so3, frameToFrameRGB, reader.getFile(), capacity, device);
+                        photoThresh, confidence, depth, icp, fastOdom, fernThresh, so3, frameToFrameRGB, reader.getFile(), capacity, device,
+                        deviceLoopClosure);
   int framesToSkip = 0, processed = 0;
   const auto t0 = std::chrono::steady_clock::now();
   while (reader.hasMore() && eFusion.getTick() < end) {
@@ -198,6 +201,7 @@ int main(int argc, char** argv) {
   const double s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   std::printf("%d frames in %.3f s (%.1f frames/s incl. log decode), %u surfels, tick %d\n", processed, s, processed / (s > 0 ? s : 1),
               eFusion.getGlobalModel().lastCount(), eFusion.getTick());
+  if (deviceLoopClosure) std::printf("deforms %d\n", eFusion.getDeforms());
   if (findArg(argc, argv, "-ply") > 0 && !iclnuim) eFusion.savePly();
   delete gt;
   return 0;  // ~ElasticFusion writes <log>.freiburg (and <log>.ply with -icl)
