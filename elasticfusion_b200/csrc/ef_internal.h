@@ -155,10 +155,7 @@ struct MapDev {
   unsigned int* clean_ctl;   // [0] tile dispenser, [1] exit tickets, [2] first tile that moves (k_clean_flags -> k_clean_move)
   uint32_t* keep_mask;       // one warp ballot per 32 surfels: the clean test's verdicts
   uint8_t* flags;         // capacity + W*H
-  // first-frame feedback buffers
-  float4 *fb_raw[3], *fb_filt[3];
-  int* fb_count;          // [2]
-  MapPose* pose;          // device
+  MapPose* pose;         // device
   int* dense_flag;        // device: 1 if the predicted image is dense enough (no fill-in)
   int* tick;              // device-resident tick
   float* nodes;           // deformation graph of the current frame, 16 floats per node

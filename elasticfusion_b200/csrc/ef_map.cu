@@ -88,6 +88,29 @@ __device__ __forceinline__ f3 normal_central(const float* depth, int rows, int c
                        (yb.z + vPos.z) / 2 - (yf.z + vPos.z) / 2);
   return normalized(cross(del_x, del_y));
 }
+// measurement geometry of pixel (i, j) of the reference's uv buffer (vertex_feedback.vert, data.vert): texel centre (tcx, tcy),
+// pixel position (x, y) and the vertex of the raw depth; add_filtered() adds the vertex of the filtered depth and its
+// normal_central at the same position
+struct PixelGeom {
+  int i, j;
+  float tcx, tcy, x, y;
+  f3 v_raw, v_filt, n_filt;
+};
+__device__ __forceinline__ PixelGeom pixel_geom(const float* depth_raw, int rows, int cols, const Cam& c, float ifx, float ify, int i, int j) {
+  PixelGeom g;
+  g.i = i;
+  g.j = j;
+  g.tcx = uv_coord(i, cols);
+  g.tcy = uv_coord(j, rows);
+  g.x = g.tcx * (float)cols;
+  g.y = g.tcy * (float)rows;
+  g.v_raw = vertex_f(depth_raw, rows, cols, i, j, g.x, g.y, c, ifx, ify);
+  return g;
+}
+__device__ __forceinline__ void add_filtered(PixelGeom& g, const float* depth_filt, int rows, int cols, const Cam& c, float ifx, float ify) {
+  g.v_filt = vertex_f(depth_filt, rows, cols, g.i, g.j, g.x, g.y, c, ifx, ify);
+  g.n_filt = normal_central(depth_filt, rows, cols, g.i, g.j, g.x, g.y, g.v_filt, c, ifx, ify);
+}
 // geometry.glsl:42-60 (ushort mm sampler, integer pixel coords)
 __device__ __forceinline__ f3 vertex_u(const uint16_t* depth, int rows, int cols, int ix, int iy, int x, int y, const Cam& c, float ifx,
                                        float ify) {
@@ -113,6 +136,18 @@ __device__ __forceinline__ unsigned int depth24(float zw) {
   if (!(zw > 0.f)) zw = 0.f;
   if (zw > 1.f) zw = 1.f;
   return (unsigned int)rintf(zw * 16777215.0f);
+}
+// vertex stage of index_map.vert / splat.vert for a camera-space point h: projection to normalised device coordinates,
+// the frustum test (false: clipped) and the window coordinates xw, yw with the NDC depth zn
+__device__ __forceinline__ bool gl_vertex(const Cam& c, int rows, int cols, float max_depth, const f3& h, float& xw, float& yw, float& zn) {
+  const float fcols = (float)cols, frows = (float)rows;
+  const float xn = ((((c.fx * h.x) / h.z) + c.cx) - (fcols * 0.5f)) / (fcols * 0.5f);
+  const float yn = ((((c.fy * h.y) / h.z) + c.cy) - (frows * 0.5f)) / (frows * 0.5f);
+  zn = h.z / max_depth;
+  if (!(xn >= -1.f && xn <= 1.f && yn >= -1.f && yn <= 1.f && zn >= -1.f && zn <= 1.f)) return false;
+  xw = (xn + 1.0f) * (fcols * 0.5f);
+  yw = (yn + 1.0f) * (frows * 0.5f);
+  return true;
 }
 
 
@@ -144,6 +179,15 @@ __device__ __forceinline__ WinAxis window_axis(float centre, float step, int n) 
   }
   return A;
 }
+// the index texels of the window spanned by two axes, cur[3 * x + y] (x outer, y inner, ascending); texels no sample lands
+// on read as empty (0)
+__device__ __forceinline__ void window_index(const uint32_t* index, int cols, const WinAxis& ax, const WinAxis& ay, uint32_t (&cur)[9]) {
+#pragma unroll
+  for (int ia = 0; ia < 3; ++ia)
+#pragma unroll
+    for (int jb = 0; jb < 3; ++jb)
+      cur[ia * 3 + jb] = (ax.m[ia] > 0 && ay.m[jb] > 0) ? index[(ay.t0 + jb) * cols + (ax.t0 + ia)] : 0u;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // pose upload: T_wc (double) -> float pose and float inverse, as the shader uniforms (GlobalModel.cpp:405,562)
@@ -162,15 +206,61 @@ __global__ void k_update_pose(MapPose* mp, const double* T) {
 // ---------------------------------------------------------------------------------------------------------------
 // single-pass exclusive scan of byte flags (decoupled look-back), persistent CTAs, device-resident length
 // ---------------------------------------------------------------------------------------------------------------
+// Decoupled look-back of one tile, run by one whole warp (k_scan_flags, k_clean_move). Tile states carry the launch's epoch
+// in their upper bits ([63:34] epoch, [33:32] status, [31:0] value), so states left by earlier scans read as "not published"
+// and nothing has to be cleared between scans. The scan starts at tile `first` with prefix `base`; tiles below `first` are
+// never read. Publishes the aggregate, then looks back for the exclusive prefix 32 predecessors at a time (status 1 =
+// aggregate only, 2 = inclusive prefix; status and value share one 64-bit word, so no fence is needed), publishes the
+// inclusive prefix and returns the exclusive one.
+__device__ __forceinline__ int lookback_prefix(unsigned long long* state, int tile, int first, int base, int aggregate, unsigned int epoch) {
+  const int lane = threadIdx.x & 31;
+  const unsigned long long tag = (unsigned long long)epoch << 34;
+  volatile unsigned long long* vstate = state;
+  if (tile == first) {
+    if (lane == 0) vstate[tile] = tag | (2ull << 32) | (unsigned int)(base + aggregate);
+    return base;
+  }
+  int prefix = 0;
+  if (lane == 0) vstate[tile] = tag | (1ull << 32) | (unsigned int)aggregate;
+  int look = tile - 1;
+  while (true) {
+    const int idx = look - lane;
+    const unsigned long long w = (idx >= first) ? vstate[idx] : (tag | (2ull << 32));
+    const unsigned int st = ((w >> 34) == (unsigned long long)epoch) ? ((unsigned int)(w >> 32) & 3u) : 0u;
+    if (__any_sync(0xffffffffu, st == 0)) continue;  // a predecessor has not published yet: re-read
+    const unsigned int m2 = __ballot_sync(0xffffffffu, st == 2);
+    const int first2 = m2 ? (__ffs(m2) - 1) : 32;
+    int val = (lane <= first2) ? (int)(unsigned int)(w & 0xffffffffull) : 0;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) val += __shfl_xor_sync(0xffffffffu, val, off);
+    prefix += val;
+    if (m2) break;
+    look -= 32;
+  }
+  if (lane == 0) vstate[tile] = tag | (2ull << 32) | (unsigned int)(prefix + aggregate);
+  return prefix;
+}
+
+// Exit of a persistent grid that draws tiles from the dispenser counter[0], called by one thread per CTA once the CTA is
+// done: it takes an exit ticket from counter[1], and the last CTA to do so re-arms both counters for the next launch and
+// gets true. FENCED: gpu-scope fences order the CTA's writes before its ticket (release) and the other CTAs' writes before
+// what the last CTA does next (acquire), for a last CTA that reads what the others wrote (k_clean_move's count).
+template <bool FENCED>
+__device__ __forceinline__ bool dispenser_exit(unsigned int* counter) {
+  if (FENCED) __threadfence();
+  if (atomicAdd(counter + 1, 1u) != gridDim.x - 1) return false;
+  if (FENCED) __threadfence();
+  counter[0] = 0u;
+  counter[1] = 0u;
+  return true;
+}
+
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_flags(const uint8_t* __restrict__ flags, const int* __restrict__ n_a,
                                                               const int* __restrict__ n_b, int* __restrict__ offsets,
                                                               unsigned long long* state, unsigned int* counter, int* total_out,
                                                               unsigned int epoch) {
-  // Tile states carry the launch's epoch in their upper bits ([63:34] epoch, [33:32] status, [31:0] value), so states left
-  // by earlier scans read as "not published" and nothing has to be cleared between scans; the tile dispenser
-  // (counter[0]) is reset by the last CTA to leave (counter[1] counts exits).
+  // tile states: see lookback_prefix; the tile dispenser (counter[0]) is reset by the last CTA to leave (dispenser_exit)
   pdl_enter();
-  const unsigned long long tag = (unsigned long long)epoch << 34;
   const int n = (n_a ? *n_a : 0) + (n_b ? *n_b : 0);
   const int num_tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
   __shared__ int s_warp[SCAN_THREADS / 32];
@@ -184,10 +274,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_flags(const uint8_t* __re
     __syncthreads();
     const int tile = s_tile;
     if (tile >= num_tiles) {
-      if (threadIdx.x == 0 && atomicAdd(counter + 1, 1u) == gridDim.x - 1) {
-        counter[0] = 0u;  // every CTA has drawn its terminating ticket: re-arm for the next scan
-        counter[1] = 0u;
-      }
+      if (threadIdx.x == 0) dispenser_exit<false>(counter);  // every CTA has drawn its terminating ticket: re-arm for the next scan
       return;
     }
     const int base = tile * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
@@ -221,32 +308,8 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_flags(const uint8_t* __re
     const int warp_excl = wid ? s_warp[wid - 1] : 0;
     const int thread_excl = warp_excl + incl - sum;
     const int aggregate = s_warp[SCAN_THREADS / 32 - 1];
-    // publish the aggregate, then look back for the exclusive prefix 32 predecessors at a time (decoupled look-back:
-    // status 1 = aggregate only, 2 = inclusive prefix; status and value share one 64-bit word, so no fence is needed)
     if (wid == 0) {
-      volatile unsigned long long* vstate = state;
-      int prefix = 0;
-      if (tile == 0) {
-        if (lane == 0) vstate[0] = tag | (2ull << 32) | (unsigned int)aggregate;
-      } else {
-        if (lane == 0) vstate[tile] = tag | (1ull << 32) | (unsigned int)aggregate;
-        int look = tile - 1;
-        while (true) {
-          const int idx = look - lane;
-          const unsigned long long w = (idx >= 0) ? vstate[idx] : (tag | (2ull << 32));
-          const unsigned int st = ((w >> 34) == (unsigned long long)epoch) ? ((unsigned int)(w >> 32) & 3u) : 0u;
-          if (__any_sync(0xffffffffu, st == 0)) continue;  // a predecessor has not published yet: re-read
-          const unsigned int m2 = __ballot_sync(0xffffffffu, st == 2);
-          const int first2 = m2 ? (__ffs(m2) - 1) : 32;
-          int val = (lane <= first2) ? (int)(unsigned int)(w & 0xffffffffull) : 0;
-#pragma unroll
-          for (int off = 16; off > 0; off >>= 1) val += __shfl_xor_sync(0xffffffffu, val, off);
-          prefix += val;
-          if (m2) break;
-          look -= 32;
-        }
-        if (lane == 0) vstate[tile] = tag | (2ull << 32) | (unsigned int)(prefix + aggregate);
-      }
+      const int prefix = lookback_prefix(state, tile, 0, 0, aggregate, epoch);
       if (lane == 0) {
         s_prefix = prefix;
         if (tile == num_tiles - 1 && total_out) *total_out = prefix + aggregate;
@@ -290,14 +353,12 @@ __global__ void k_init_scatter(const uint8_t* __restrict__ rgb, const float* __r
   if (blockIdx.x == 0 && threadIdx.x == 0) *count = min(*raw_total, capacity);
   for (int d = blockIdx.x * blockDim.x + threadIdx.x; d < n; d += gridDim.x * blockDim.x) {
     const int i = d / rows, j = d - i * rows;
-    const float tcx = uv_coord(i, cols), tcy = uv_coord(j, rows);
-    const float x = tcx * (float)cols, y = tcy * (float)rows;
     if (f_raw[d]) {
       const int k = off_raw[d];
       if (k < capacity) {
-        const f3 v = vertex_f(depth_raw, rows, cols, i, j, x, y, c, ifx, ify);
+        const PixelGeom g = pixel_geom(depth_raw, rows, cols, c, ifx, ify, i, j);
         const uint8_t* px = rgb + ((size_t)j * cols + i) * 3;
-        pos_conf[k] = make_float4(v.x, v.y, v.z, confidence(x, y, 1.0f, c.cx, c.cy));
+        pos_conf[k] = make_float4(g.v_raw.x, g.v_raw.y, g.v_raw.z, confidence(g.x, g.y, 1.0f, c.cx, c.cy));
         // init_unstable.vert: colour.y = 0 (unused), colour.z = 1 (init time); colour.w = time from vertex_feedback.vert
         color_time[k] = make_float4(encode_color_bytes(px[0], px[1], px[2]), 0.f, 1.f, (float)time);
       }
@@ -305,9 +366,9 @@ __global__ void k_init_scatter(const uint8_t* __restrict__ rgb, const float* __r
     if (f_filt[d]) {
       const int k = off_filt[d];
       if (k < capacity) {
-        const f3 v = vertex_f(depth_filt, rows, cols, i, j, x, y, c, ifx, ify);
-        const f3 nrm = normal_central(depth_filt, rows, cols, i, j, x, y, v, c, ifx, ify);
-        norm_rad[k] = make_float4(nrm.x, nrm.y, nrm.z, get_radius(v.z, nrm.z, ifx, ify));
+        PixelGeom g = pixel_geom(depth_raw, rows, cols, c, ifx, ify, i, j);  // (the raw vertex goes unused here)
+        add_filtered(g, depth_filt, rows, cols, c, ifx, ify);
+        norm_rad[k] = make_float4(g.n_filt.x, g.n_filt.y, g.n_filt.z, get_radius(g.v_filt.z, g.n_filt.z, ifx, ify));
       }
     }
   }
@@ -331,7 +392,6 @@ __global__ void __launch_bounds__(256, 5) k_index_scatter(const float4* __restri
   pdl_enter();
   const int n_map = *count;
   const int n = (MODE == 2) ? min(*vis_count, vis_capacity) : n_map;
-  const float fcols = (float)cols, frows = (float)rows;
   // Two surfels per thread and round, in three phases -- 4 loads, 2 projections + 2 z-buffer reads, <= 2 atomics -- so that a
   // thread has independent requests in flight instead of a chain of three (one surfel at a time: 40 us for 5 M surfels,
   // long-scoreboard 20 per issue at 39 % of the DRAM roof). One resident wave of 5 CTAs per SM (<= 51 registers); a small map
@@ -367,12 +427,8 @@ __global__ void __launch_bounds__(256, 5) k_index_scatter(const float4* __restri
       const f3 h = xform(mp->t_inv, mk3(pc[u].x, pc[u].y, pc[u].z));
       if (h.z > max_depth || h.z < 0) continue;
       if ((float)time - last_time[u] > (float)time_delta) continue;
-      const float xn = ((((c.fx * h.x) / h.z) + c.cx) - (fcols * 0.5f)) / (fcols * 0.5f);
-      const float yn = ((((c.fy * h.y) / h.z) + c.cy) - (frows * 0.5f)) / (frows * 0.5f);
-      const float zn = h.z / max_depth;
-      if (!(xn >= -1.f && xn <= 1.f && yn >= -1.f && yn <= 1.f && zn >= -1.f && zn <= 1.f)) continue;
-      const float xw = (xn + 1.0f) * (fcols * 0.5f);
-      const float yw = (yn + 1.0f) * (frows * 0.5f);
+      float xw, yw, zn;
+      if (!gl_vertex(c, rows, cols, max_depth, h, xw, yw, zn)) continue;
       const int px = point_pixel(xw), py = point_pixel(yw);
       if (px < 0 || py < 0 || px >= cols || py >= rows) continue;
       const unsigned int d24 = depth24(0.5f * zn + 0.5f);
@@ -463,20 +519,16 @@ __device__ __host__ __forceinline__ Quarter quarter_of(int time, int rows, int c
 }
 
 // measurement geometry of pixel (i,j) as data.vert builds it; returns false if the pixel takes no part this frame
-__device__ __forceinline__ bool fuse_active(const FuseArgs& a, int i, int j, float& tcx, float& tcy, float& x, float& y, f3& vPosLocal) {
-  tcx = uv_coord(i, a.cols);
-  tcy = uv_coord(j, a.rows);
-  x = tcx * (float)a.cols;
-  y = tcy * (float)a.rows;
-  const float ftime = (float)a.time;
-  if (!((int)x % 2 == (int)ftime % 2 && (int)y % 2 == (int)ftime % 2)) return false;
+__device__ __forceinline__ bool fuse_active(const FuseArgs& a, int i, int j, PixelGeom& g) {
   const float ifx = (float)(1.0 / (double)a.c.fx), ify = (float)(1.0 / (double)a.c.fy);
-  vPosLocal = vertex_f(a.depth_raw, a.rows, a.cols, i, j, x, y, a.c, ifx, ify);
+  g = pixel_geom(a.depth_raw, a.rows, a.cols, a.c, ifx, ify, i, j);
+  const float ftime = (float)a.time;
+  if (!((int)g.x % 2 == (int)ftime % 2 && (int)g.y % 2 == (int)ftime % 2)) return false;
   const int il = max(i - 1, 0), ir = min(i + 1, a.cols - 1), ju = max(j - 1, 0), jd = min(j + 1, a.rows - 1);
   if (a.depth_raw[(size_t)j * a.cols + il] == 0 || a.depth_raw[(size_t)ju * a.cols + i] == 0 ||
       a.depth_raw[(size_t)j * a.cols + ir] == 0 || a.depth_raw[(size_t)jd * a.cols + i] == 0)
     return false;
-  return (vPosLocal.z > 0 && vPosLocal.z <= a.max_depth);
+  return (g.v_raw.z > 0 && g.v_raw.z <= a.max_depth);
 }
 
 constexpr uint32_t ASSOC_NONE = 0xffffffffu, ASSOC_NEW = 0xfffffffeu;
@@ -490,14 +542,13 @@ __global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint
   for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x) {
     const int i = 2 * (q / Q.nj) + Q.p, j = 2 * (q % Q.nj) + Q.p;
     const uint32_t d = (uint32_t)i * a.rows + j;  // draw index in the reference's uv buffer
-    float tcx, tcy, x, y;
-    f3 vPosLocal;
+    PixelGeom g;
     uint32_t res = ASSOC_NONE;
     uint8_t is_new = 0;
-    if (fuse_active(a, i, j, tcx, tcy, x, y, vPosLocal)) {
+    if (fuse_active(a, i, j, g)) {
       const float ifx = (float)(1.0 / (double)a.c.fx), ify = (float)(1.0 / (double)a.c.fy);
-      const f3 vPos_f = vertex_f(a.depth_filt, a.rows, a.cols, i, j, x, y, a.c, ifx, ify);
-      const f3 vNormLocal = normal_central(a.depth_filt, a.rows, a.cols, i, j, x, y, vPos_f, a.c, ifx, ify);
+      add_filtered(g, a.depth_filt, a.rows, a.cols, a.c, ifx, ify);
+      const f3 vNormLocal = g.n_filt;
       const float fcols = (float)a.cols, frows = (float)a.rows;
       int counter = 0;
       uint32_t best = 0;
@@ -505,20 +556,16 @@ __global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint
       const float indexXStep = (1.0f / (fcols * scale)) * 0.5f;
       const float indexYStep = (1.0f / (frows * scale)) * 0.5f;
       float bestDist = 1000;
-      const float xl = (x - a.c.cx) * ifx;
-      const float yl = (y - a.c.cy) * ify;
+      const float xl = (g.x - a.c.cx) * ifx;
+      const float yl = (g.y - a.c.cy) * ify;
       const float lambda = sqrtf(xl * xl + yl * yl + 1);
       const f3 ray = mk3(xl, yl, 1);
       // duplicates of a texel cannot change the outcome (strict `dist < bestDist`), so each distinct texel is visited once,
       // in the reference's order (x outer, y inner, ascending). All nine index texels are fetched first, then the attributes
       // of the occupied ones column by column: four dependent memory round trips instead of one or two per texel.
-      const WinAxis ax = window_axis(tcx, indexXStep, a.cols), ay = window_axis(tcy, indexYStep, a.rows);
+      const WinAxis ax = window_axis(g.tcx, indexXStep, a.cols), ay = window_axis(g.tcy, indexYStep, a.rows);
       uint32_t cur[9];
-#pragma unroll
-      for (int ia = 0; ia < 3; ++ia)
-#pragma unroll
-        for (int jb = 0; jb < 3; ++jb)
-          cur[ia * 3 + jb] = (ax.m[ia] > 0 && ay.m[jb] > 0) ? a.index[(ay.t0 + jb) * a.cols + (ax.t0 + ia)] : 0u;
+      window_index(a.index, a.cols, ax, ay, cur);
 #pragma unroll
       for (int ia = 0; ia < 3; ++ia) {
         float4 vc[3], nr[3];
@@ -533,7 +580,7 @@ __global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint
         for (int jb = 0; jb < 3; ++jb) {
           const uint32_t current = cur[ia * 3 + jb];
           if (current > 0U) {
-            if (fabsf((vc[jb].z * lambda) - (vPosLocal.z * lambda)) < 0.05f) {
+            if (fabsf((vc[jb].z * lambda) - (g.v_raw.z * lambda)) < 0.05f) {
               const float dist = norm(cross(ray, mk3(vc[jb].x, vc[jb].y, vc[jb].z))) / norm(ray);
               const f3 nrm = mk3(nr[jb].x, nr[jb].y, nr[jb].z);
               const float ang = acosf(dot(nrm, vNormLocal) / (norm(nrm) * norm(vNormLocal)));
@@ -561,18 +608,15 @@ __global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint
 
 __device__ __forceinline__ void fuse_measurement(const FuseArgs& a, const MapPose* mp, float weighting, int i, int j, float4& pos, float4& col,
                                                  float4& nr) {
-  const float tcx = uv_coord(i, a.cols), tcy = uv_coord(j, a.rows);
-  const float x = tcx * (float)a.cols, y = tcy * (float)a.rows;
   const float ifx = (float)(1.0 / (double)a.c.fx), ify = (float)(1.0 / (double)a.c.fy);
-  const f3 vPosLocal = vertex_f(a.depth_raw, a.rows, a.cols, i, j, x, y, a.c, ifx, ify);
-  const f3 vg = xform(mp->pose, vPosLocal);
-  const f3 vPos_f = vertex_f(a.depth_filt, a.rows, a.cols, i, j, x, y, a.c, ifx, ify);
-  const f3 vNormLocal = normal_central(a.depth_filt, a.rows, a.cols, i, j, x, y, vPos_f, a.c, ifx, ify);
-  const f3 ng = rot(mp->pose, vNormLocal);
+  PixelGeom g = pixel_geom(a.depth_raw, a.rows, a.cols, a.c, ifx, ify, i, j);
+  const f3 vg = xform(mp->pose, g.v_raw);
+  add_filtered(g, a.depth_filt, a.rows, a.cols, a.c, ifx, ify);
+  const f3 ng = rot(mp->pose, g.n_filt);
   const uint8_t* px = a.rgb + ((size_t)j * a.cols + i) * 3;
-  pos = make_float4(vg.x, vg.y, vg.z, confidence(x, y, weighting, a.c.cx, a.c.cy));
+  pos = make_float4(vg.x, vg.y, vg.z, confidence(g.x, g.y, weighting, a.c.cx, a.c.cy));
   col = make_float4(encode_color_bytes(px[0], px[1], px[2]), 0.f, (float)a.time, 0.f);
-  nr = make_float4(ng.x, ng.y, ng.z, get_radius(vPos_f.z, vNormLocal.z, ifx, ify));
+  nr = make_float4(ng.x, ng.y, ng.z, get_radius(g.v_filt.z, g.n_filt.z, ifx, ify));
 }
 
 // one associated pixel q of the quarter grid: a new surfel goes to new_*[k_new]; the pixel that owns a matched surfel's winner slot
@@ -778,11 +822,7 @@ __device__ __forceinline__ bool clean_test(const CleanArgs& a, const MapPose* mp
     // weighted by the number of float-loop samples that land on it. Index texels first, attributes of the occupied ones after.
     const WinAxis ax = window_axis(x / fcols, indexXStep, a.cols), ay = window_axis(y / frows, indexYStep, a.rows);
     uint32_t cur[9];
-#pragma unroll
-    for (int ia = 0; ia < 3; ++ia)
-#pragma unroll
-      for (int jb = 0; jb < 3; ++jb)
-        cur[ia * 3 + jb] = (ax.m[ia] > 0 && ay.m[jb] > 0) ? a.index[(ay.t0 + jb) * a.cols + (ax.t0 + ia)] : 0u;
+    window_index(a.index, a.cols, ax, ay, cur);
 #pragma unroll
     for (int ia = 0; ia < 3; ++ia) {
       float4 vcs[3], cts[3];
@@ -928,7 +968,6 @@ __global__ void __launch_bounds__(CC_THREADS) k_clean_move(CleanArgs a, const Ma
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n_old = *count, total = n_old + *new_count;
   const int num_tiles = (total + CC_TILE - 1) / CC_TILE;
-  const unsigned long long tag = (unsigned long long)epoch << 34;
   unsigned int* counter = ctl;
   // tiles below `first` are full and stay where they are: the compaction starts there with prefix first * CC_TILE
   const unsigned int first_u = *(volatile unsigned int*)(ctl + 2);
@@ -1023,30 +1062,7 @@ __global__ void __launch_bounds__(CC_THREADS) k_clean_move(CleanArgs a, const Ma
       }
       if (lane < CC_ITEMS * (CC_THREADS / 32)) S.warp_excl[lane] = incl - c;
       const int aggregate = __shfl_sync(0xffffffffu, incl, 31);
-      volatile unsigned long long* vstate = state;
-      int prefix = first * CC_TILE;
-      if (cur == first) {
-        if (lane == 0) vstate[cur] = tag | (2ull << 32) | (unsigned int)(prefix + aggregate);
-      } else {
-        prefix = 0;
-        if (lane == 0) vstate[cur] = tag | (1ull << 32) | (unsigned int)aggregate;
-        int look = cur - 1;
-        while (true) {
-          const int idx = look - lane;
-          const unsigned long long w = (idx >= first) ? vstate[idx] : (tag | (2ull << 32));
-          const unsigned int stt = ((w >> 34) == (unsigned long long)epoch) ? ((unsigned int)(w >> 32) & 3u) : 0u;
-          if (__any_sync(0xffffffffu, stt == 0)) continue;
-          const unsigned int m2 = __ballot_sync(0xffffffffu, stt == 2);
-          const int first2 = m2 ? (__ffs(m2) - 1) : 32;
-          int val = (lane <= first2) ? (int)(unsigned int)(w & 0xffffffffull) : 0;
-#pragma unroll
-          for (int off = 16; off > 0; off >>= 1) val += __shfl_xor_sync(0xffffffffu, val, off);
-          prefix += val;
-          if (m2) break;
-          look -= 32;
-        }
-        if (lane == 0) vstate[cur] = tag | (2ull << 32) | (unsigned int)(prefix + aggregate);
-      }
+      const int prefix = lookback_prefix(state, cur, first, first * CC_TILE, aggregate, epoch);
       if (lane == 0) {
         S.prefix = prefix;
         S.aggregate = aggregate;
@@ -1075,19 +1091,13 @@ __global__ void __launch_bounds__(CC_THREADS) k_clean_move(CleanArgs a, const Ma
     stage ^= 1;
   }
   // leave: the last CTA to draw its terminating ticket re-arms the dispenser and publishes the counts
-  if (tid == 0) {
-    __threadfence();
-    if (atomicAdd(counter + 1, 1u) == gridDim.x - 1) {
-      __threadfence();
-      counter[0] = 0u;
-      counter[1] = 0u;
-      counter[2] = 0xffffffffu;
-      if (first < num_tiles) {  // (otherwise nothing was culled and nothing is new: the count stands)
-        const int kept = *(volatile int*)total_out;
-        *count = kept < capacity ? kept : capacity;
-      }
-      *new_count = 0;
+  if (tid == 0 && dispenser_exit<true>(counter)) {
+    counter[2] = 0xffffffffu;
+    if (first < num_tiles) {  // (otherwise nothing was culled and nothing is new: the count stands)
+      const int kept = *(volatile int*)total_out;
+      *count = kept < capacity ? kept : capacity;
     }
+    *new_count = 0;
   }
 }
 
@@ -1112,14 +1122,11 @@ __device__ __forceinline__ f3 project_image(const Cam& c, const f3& p) { return 
 
 __device__ __forceinline__ bool splat_vertex(const RayArgs& a, const MapPose* mp, const float4& pc, const float4& ct, const float4* norm_rad,
                                              int id, Splat& sp) {
-  const float fcols = (float)a.cols, frows = (float)a.rows;
   const f3 h = xform(mp->t_inv, mk3(pc.x, pc.y, pc.z));
   if (h.z > a.max_depth || h.z < 0 || pc.w < a.conf_threshold || (float)a.time - ct.w > (float)a.time_delta || ct.w > (float)a.max_time)
     return false;
-  const float xn = ((((a.c.fx * h.x) / h.z) + a.c.cx) - (fcols * 0.5f)) / (fcols * 0.5f);
-  const float yn = ((((a.c.fy * h.y) / h.z) + a.c.cy) - (frows * 0.5f)) / (frows * 0.5f);
-  const float zn = h.z / a.max_depth;
-  if (!(xn >= -1.f && xn <= 1.f && yn >= -1.f && yn <= 1.f && zn >= -1.f && zn <= 1.f)) return false;
+  float zn;
+  if (!gl_vertex(a.c, a.rows, a.cols, a.max_depth, h, sp.xw, sp.yw, zn)) return false;
   const float4 nr = norm_rad[id];
   sp.pos = h;
   sp.conf = pc.w;
@@ -1135,8 +1142,6 @@ __device__ __forceinline__ bool splat_vertex(const RayArgs& a, const MapPose* mp
   if (!(size >= 1.0f)) size = 1.0f;
   if (size > 2047.0f) size = 2047.0f;
   sp.size = size;
-  sp.xw = (xn + 1.0f) * (fcols * 0.5f);
-  sp.yw = (yn + 1.0f) * (frows * 0.5f);
   return true;
 }
 
@@ -1486,8 +1491,7 @@ int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_
   const size_t tiles = (max_items + SCAN_TILE - 1) / SCAN_TILE + 1;
   MapBuffers& B = mb(ctx);
   RC(next_scan_epoch(ctx, B));
-  size_t nb = tiles < (size_t)ctx->num_sms * 4 ? tiles : (size_t)ctx->num_sms * 4;
-  EF_LAUNCH(ctx, k_scan_flags, (int)nb, SCAN_THREADS, 0, flags, n_a, n_b, offsets, (unsigned long long*)m.scan_tile_state, m.scan_counter, total,
+  EF_LAUNCH(ctx, k_scan_flags, wave_blocks(ctx, tiles, 4, 1), SCAN_THREADS, 0, flags, n_a, n_b, offsets, (unsigned long long*)m.scan_tile_state, m.scan_counter, total,
             B.scan_epoch);
   CHECK_LAST();
   return 0;
@@ -1537,15 +1541,9 @@ int map_predict_indices_async(EfContext* ctx, int time, float max_depth, int tim
   if (vis_mode == 2 && !ctx->vis_pending) vis_mode = 0;
   if (vis_mode == 1) ctx->vis_pending = true;
   if (vis_mode == 2) ctx->vis_pending = false;
-  if (vis_mode == 1)
-    EF_LAUNCH(ctx, k_index_scatter<1>, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols,
-              cam_of(ctx), m.zbuf, m.vis_list, m.vis_count, m.capacity);
-  else if (vis_mode == 2)
-    EF_LAUNCH(ctx, k_index_scatter<2>, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols,
-              cam_of(ctx), m.zbuf, m.vis_list, m.vis_count, m.capacity);
-  else
-    EF_LAUNCH(ctx, k_index_scatter<0>, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols,
-              cam_of(ctx), m.zbuf, (uint32_t*)nullptr, (int*)nullptr, 0);
+  const auto scatter = vis_mode == 1 ? k_index_scatter<1> : vis_mode == 2 ? k_index_scatter<2> : k_index_scatter<0>;  // (mode 0 never reads the list)
+  EF_LAUNCH(ctx, scatter, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols, cam_of(ctx),
+            m.zbuf, m.vis_list, m.vis_count, m.capacity);
   EF_LAUNCH(ctx, k_index_resolve, wave_blocks(ctx, n), 256, 0, m.pos_conf, m.color_time, m.norm_rad, m.pose, n, m.zbuf, ctx->tex.index,
             ctx->tex.vert_conf, ctx->tex.color_time, ctx->tex.norm_rad, vis_mode == 2 ? m.vis_count : (int*)nullptr);
   CHECK_LAST();
@@ -1614,22 +1612,12 @@ int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_del
   RC(next_scan_epoch(ctx, B));
   // grids never depend on a surfel count the host would have to read back: the test strides over the tiles, the movers draw
   // tiles from a dispenser (one resident wave: four 49 KB CTAs per SM)
-  size_t nb = (size_t)ctx->num_sms * 4;
-  if (nb > tiles) nb = tiles;
-  if (nb < 1) nb = 1;
-  size_t nbf = (size_t)ctx->num_sms * 2;
-  if (nbf > tiles) nbf = tiles;
-  if (nbf < 1) nbf = 1;
-  EF_LAUNCH(ctx, k_clean_flags, (int)nbf, CF_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos, m.new_col, m.new_nr,
-            m.new_count, m.keep_mask, m.clean_ctl);
-  if (n_nodes > 0)
-    EF_LAUNCH(ctx, k_clean_move<true>, (int)nb, CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
-              m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
-              B.scan_epoch);
-  else
-    EF_LAUNCH(ctx, k_clean_move<false>, (int)nb, CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
-              m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
-              B.scan_epoch);
+  EF_LAUNCH(ctx, k_clean_flags, wave_blocks(ctx, tiles, 2, 1), CF_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
+            m.new_col, m.new_nr, m.new_count, m.keep_mask, m.clean_ctl);
+  const auto move = n_nodes > 0 ? k_clean_move<true> : k_clean_move<false>;
+  EF_LAUNCH(ctx, move, wave_blocks(ctx, tiles, 4, 1), CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count,
+            m.new_pos, m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
+            B.scan_epoch);
   CHECK_LAST();
   return 0;
 }
@@ -1647,16 +1635,19 @@ int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int
   a.max_time = max_time;
   a.time_delta = time_delta;
   EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.zbuf);
+  // mode 0: the predicted model, 1: the old model (loop closure), 2: the synthesised depth alone
   Textures& t = ctx->tex;
-  if (mode == 0)
-    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.image, t.vertex, t.normal,
-              t.time, (float*)nullptr);
-  else if (mode == 1)
-    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, t.old_image, t.old_vertex,
-              t.old_normal, t.old_time, (float*)nullptr);
-  else
-    EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, (uchar4*)nullptr,
-              (float4*)nullptr, (float4*)nullptr, (uint16_t*)nullptr, t.synth_depth);
+  struct Out {
+    uchar4* image;
+    float4 *vertex, *normal;
+    uint16_t* time;
+    float* depth;
+  };
+  const Out o = mode == 0 ? Out{t.image, t.vertex, t.normal, t.time, nullptr}
+              : mode == 1 ? Out{t.old_image, t.old_vertex, t.old_normal, t.old_time, nullptr}
+                          : Out{nullptr, nullptr, nullptr, nullptr, t.synth_depth};
+  EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, o.image, o.vertex, o.normal,
+            o.time, o.depth);
   CHECK_LAST();
   return 0;
 }
