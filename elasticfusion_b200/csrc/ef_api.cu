@@ -138,7 +138,6 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   }
   g.break_level = -1;
   g.weighting = 1.0f;
-  g.flat_n = od.level_start[NUM_PYRS];
   CU(cudaMemcpyAsync(od.gn, &g, sizeof(g), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
@@ -420,6 +419,7 @@ extern "C" int ef_upload(EfContext* ctx, int32_t id, int32_t level, const void* 
   RC(ef_buffer(ctx, id, level, &p, &b));
   if (bytes > b || !host) return EF_EINVAL;
   CU(cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if (id == EF_BUF_IMAGE) RC(map_dense_enough_async(ctx));  // the next frame's fill-in choice follows the uploaded image
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
@@ -699,8 +699,10 @@ extern "C" int ef_map_fill_in(EfContext* ctx, int32_t pass_geom, int32_t pass_im
 }
 extern "C" int ef_dense_enough(EfContext* ctx, int32_t* out) {
   if (!ctx || !out) return EF_EINVAL;
-  RC(map_dense_enough_async(ctx));
-  return read_count(ctx, ctx->map.dense_flag, out);
+  int lit = 0;  // counted by the mode-0 raycast (or the upload) that wrote the predicted image
+  RC(read_count(ctx, ctx->map.dense_count, &lit));
+  *out = dense_enough_of(lit, ctx->map.rows, ctx->map.cols) ? 1 : 0;
+  return 0;
 }
 extern "C" int ef_map_count(EfContext* ctx, int32_t* count) {
   if (!ctx || !count) return EF_EINVAL;
@@ -739,8 +741,8 @@ extern "C" int ef_map_upload(EfContext* ctx, const float* in12, int32_t count) {
 // ---------------------------------------------------------------------------------------------------------------
 // ElasticFusion::predict, reference Core/ElasticFusion.cpp:621-653 (lost == false, lastFrameRecovery == false)
 static int predict_async(EfContext* ctx) {
-  RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick, ctx->cfg.time_delta, 0));
-  return map_fill_in_async(ctx, false, ctx->frame_to_frame_rgb);
+  return map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick, ctx->cfg.time_delta, 0,
+                           ctx->frame_to_frame_rgb ? 1 : 0);
 }
 
 extern "C" int ef_predict(EfContext* ctx) {
@@ -895,8 +897,7 @@ static int frame_begin_device(EfContext* ctx, const uint8_t* rgb_dev, const uint
   OdomDev& od = ctx->odom[0];
   if (!in_T_wc) {
     // ElasticFusion.cpp:302-323. The fill-in decision stays on the device: both candidate inputs are handed to the
-    // pyramid kernels together with the flag.
-    RC(map_dense_enough_async(ctx));
+    // pyramid kernels together with the lit-sample count that the raycast writing the image (or its upload) left.
     RC(map_select_model_inputs(ctx));
     // initRGB's depth half (populateRGBDData -> verticesToDepth(vmaps_tmp), RGBDOdometry.cpp:212-222) reads the SAME
     // vmaps_tmp initICPModel just filled, so in frame-to-model mode nextDepth is identical to lastDepth: alias it for

@@ -128,4 +128,83 @@ __device__ __forceinline__ bool last_block_done(unsigned int* counter) {
   return is_last;
 }
 
+// Order-preserving compaction in one pass (k_scan_flags, k_clean_move, k_fuse_update, k_sobel_cand): a persistent grid draws tiles
+// in order from a dispenser, scans each tile inside the CTA (block_exclusive_scan) and takes the tile's prefix from its predecessors.
+//
+// Decoupled look-back of one tile, run by one whole warp. Tile states carry the launch's epoch
+// in their upper bits ([63:34] epoch, [33:32] status, [31:0] value), so states left by earlier scans read as "not published"
+// and nothing has to be cleared between scans. The scan starts at tile `first` with prefix `base`; tiles below `first` are
+// never read. Publishes the aggregate, then looks back for the exclusive prefix 32 predecessors at a time (status 1 =
+// aggregate only, 2 = inclusive prefix; status and value share one 64-bit word, so no fence is needed), publishes the
+// inclusive prefix and returns the exclusive one.
+__device__ __forceinline__ int lookback_prefix(unsigned long long* state, int tile, int first, int base, int aggregate, unsigned int epoch) {
+  const int lane = threadIdx.x & 31;
+  const unsigned long long tag = (unsigned long long)epoch << 34;
+  volatile unsigned long long* vstate = state;
+  if (tile == first) {
+    if (lane == 0) vstate[tile] = tag | (2ull << 32) | (unsigned int)(base + aggregate);
+    return base;
+  }
+  int prefix = 0;
+  if (lane == 0) vstate[tile] = tag | (1ull << 32) | (unsigned int)aggregate;
+  int look = tile - 1;
+  while (true) {
+    const int idx = look - lane;
+    const unsigned long long w = (idx >= first) ? vstate[idx] : (tag | (2ull << 32));
+    const unsigned int st = ((w >> 34) == (unsigned long long)epoch) ? ((unsigned int)(w >> 32) & 3u) : 0u;
+    if (__any_sync(0xffffffffu, st == 0)) continue;  // a predecessor has not published yet: re-read
+    const unsigned int m2 = __ballot_sync(0xffffffffu, st == 2);
+    const int first2 = m2 ? (__ffs(m2) - 1) : 32;
+    int val = (lane <= first2) ? (int)(unsigned int)(w & 0xffffffffull) : 0;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) val += __shfl_xor_sync(0xffffffffu, val, off);
+    prefix += val;
+    if (m2) break;
+    look -= 32;
+  }
+  if (lane == 0) vstate[tile] = tag | (2ull << 32) | (unsigned int)(prefix + aggregate);
+  return prefix;
+}
+
+// Exit of a persistent grid that draws tiles from the dispenser counter[0], called by one thread per CTA once the CTA is
+// done: it takes an exit ticket from counter[1], and the last CTA to do so re-arms both counters for the next launch and
+// gets true. FENCED: gpu-scope fences order the CTA's writes before its ticket (release) and the other CTAs' writes before
+// what the last CTA does next (acquire), for a last CTA that reads what the others wrote (k_clean_move's count).
+template <bool FENCED>
+__device__ __forceinline__ bool dispenser_exit(unsigned int* counter) {
+  if (FENCED) __threadfence();
+  if (atomicAdd(counter + 1, 1u) != gridDim.x - 1) return false;
+  if (FENCED) __threadfence();
+  counter[0] = 0u;
+  counter[1] = 0u;
+  return true;
+}
+
+// Exclusive scan of one int per thread over a CTA of THREADS threads (a multiple of 32, at most 1024); also returns the CTA
+// total in `aggregate`. Every thread of the CTA must call it; s_warp holds THREADS / 32 ints and may be reused after the next barrier.
+template <int THREADS>
+__device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int& aggregate) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int incl = v;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, off);
+    if (lane >= off) incl += t;
+  }
+  if (lane == 31) s_warp[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    int w = (lane < THREADS / 32) ? s_warp[lane] : 0;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, w, off);
+      if (lane >= off) w += t;
+    }
+    if (lane < THREADS / 32) s_warp[lane] = w;  // inclusive over warps
+  }
+  __syncthreads();
+  aggregate = s_warp[THREADS / 32 - 1];
+  return (wid ? s_warp[wid - 1] : 0) + incl - v;
+}
+
 }  // namespace ef

@@ -15,6 +15,12 @@ constexpr int RED_THREADS = 256;     // threads per reduction CTA
 constexpr int MAX_RED_BLOCKS = 1184; // 8 resident 256-thread CTAs per SM on up to 148 SMs (H100: 132)
 constexpr int PARTIAL_STRIDE = 64;   // floats per CTA partial: [0,29) geometric system, [32,61) photometric system
 constexpr int MAX_TRACE = 48;
+constexpr int DENSE_FACTOR = 20;  // ElasticFusion::denseEnough decimates the predicted image by 20 (ElasticFusion.cpp:258)
+
+// ElasticFusion::denseEnough (ElasticFusion.cpp:256-268) from the number of lit samples of the decimated image
+__host__ __device__ inline bool dense_enough_of(int lit, int rows, int cols) {
+  return (float)lit / (float)((rows / DENSE_FACTOR) * (cols / DENSE_FACTOR)) > 0.75f;
+}
 constexpr int MAX_RGB_BLOCKS = 160;
 
 // reference DataTerm (Core/Cuda/types.cuh:79-84): 16 bytes, bool widened to int32
@@ -52,7 +58,6 @@ struct GNState {
   double Kd[NUM_PYRS][9], Kinvd[NUM_PYRS][9];  // per-level K (float intrinsics / 2^level, widened) and its inverse
   int trace_n;
   int cand_base[NUM_PYRS + 1];  // photometric candidates of level L live in cand[cand_base[L], cand_base[L+1])
-  int flat_n;                   // total pixels over the three levels
   float rgbErrBuf[2];           // rgbError of the previous / current iteration (double-buffered across CTAs)
   float weighting;  // velocity weighting for fusion (ElasticFusion.cpp:369-383)
   long long dbg[40];  // phase timestamps (%globaltimer) of levels 0 and 1 when built with -DEF_PROFILE_PHASES
@@ -154,9 +159,8 @@ struct MapDev {
   int* vis_count;
   unsigned int* clean_ctl;   // [0] tile dispenser, [1] exit tickets, [2] first tile that moves (k_clean_flags -> k_clean_move)
   uint32_t* keep_mask;       // one warp ballot per 32 surfels: the clean test's verdicts
-  uint8_t* flags;         // capacity + W*H
   MapPose* pose;         // device
-  int* dense_flag;        // device: 1 if the predicted image is dense enough (no fill-in)
+  int* dense_count;       // device: lit samples of the predicted image's decimation (dense_enough_of gives the flag)
   int* tick;              // device-resident tick
   float* nodes;           // deformation graph of the current frame, 16 floats per node
   LoopDev* loop;
@@ -403,8 +407,13 @@ int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba);
 // ef_map.cu: the surfel map
 int alloc_map(EfContext* ctx);
 void map_free_host(EfContext* ctx);
-int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_b, size_t max_items, int* offsets, int* total);
-void scan_scratch(EfContext* ctx, uint8_t** flags, int** offsets);
+// look-back tile states, tile dispenser and a fresh epoch for one order-preserving compaction on ctx->stream (lookback_prefix)
+struct ScanSlot {
+  unsigned long long* state;
+  unsigned int* counter;
+  unsigned int epoch;
+};
+int scan_slot(EfContext* ctx, ScanSlot* out);
 int map_initialise_async(EfContext* ctx);
 int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
 int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, int time_delta, int vis_mode = 0);
@@ -413,7 +422,8 @@ int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int t
 int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);
 int map_set_graph_device(EfContext* ctx, const float* nodes16_dev, int n_nodes);
 int map_sample_graph_async(EfContext* ctx);
-int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode);
+// mode 0 also recounts dense_count; fill_in >= 0 (mode 0 only) also runs the fill-in in the same pass, with pass_img = fill_in
+int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode, int fill_in = -1);
 int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
 int map_dense_enough_async(EfContext* ctx);
 int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);

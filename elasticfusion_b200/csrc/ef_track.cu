@@ -317,11 +317,11 @@ __global__ void k_pyr_down_depth_image(const float* __restrict__ d0, float* __re
 // separate kernels remain for the stage API and the trackers that initialise only one half.
 __global__ void k_model_level0(const float4* __restrict__ vtxA, const float4* __restrict__ nrmA, const float4* __restrict__ vtxB,
                                const float4* __restrict__ nrmB, const uchar4* __restrict__ rgbaA, const uchar4* __restrict__ rgbaB,
-                               const int* __restrict__ dense_flag, int forceB_rgb, int rows, int cols, float cutoff, float4* __restrict__ vmaps_tmp,
+                               const int* __restrict__ dense_count, int forceB_rgb, int rows, int cols, float cutoff, float4* __restrict__ vmaps_tmp,
                                float* __restrict__ vmap, float* __restrict__ nmap, float* __restrict__ depth, uint8_t* __restrict__ image) {
   pdl_enter();
   const size_t n = (size_t)rows * cols;
-  const bool useB = dense_flag && (*dense_flag == 0);
+  const bool useB = dense_count && !dense_enough_of(*dense_count, rows, cols);
   const float4* __restrict__ vtx = useB ? vtxB : vtxA;
   const float4* __restrict__ nrm = useB ? nrmB : nrmA;
   const uchar4* __restrict__ rgba = (forceB_rgb || useB) ? rgbaB : rgbaA;
@@ -404,56 +404,78 @@ struct SobelArgs {
   int start[NUM_PYRS + 1];
   float minScale[NUM_PYRS];
 };
-__global__ void k_sobel_cand(SobelArgs a, uint8_t* __restrict__ flags) {
+// A persistent grid over tiles of SC_THREADS pixels, drawn in order from the dispenser counter[0]: a candidate takes its slot in
+// the list from its tile's exclusive prefix (lookback_prefix), so the list keeps the flat pixel order (level 0, 1, 2) without a
+// separate scan. The first pixel of each level publishes the level's start, the last tile the total.
+constexpr int SC_THREADS = 256;
+__global__ void __launch_bounds__(SC_THREADS) k_sobel_cand(SobelArgs a, int4* __restrict__ cand, GNState* gn, unsigned long long* state,
+                                                          unsigned int* counter, unsigned int epoch) {
   pdl_enter();
   const float gsx[9] = {(float)0.52201, (float)0.00000, (float)-0.52201, (float)0.79451, (float)-0.00000,
                         (float)-0.79451, (float)0.52201, (float)0.00000, (float)-0.52201};
   const float gsy[9] = {(float)0.52201, (float)0.79451, (float)0.52201, (float)0.00000, (float)0.00000,
                         (float)0.00000, (float)-0.52201, (float)-0.79451, (float)-0.52201};
   const int total = a.start[NUM_PYRS];
-  for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < total; f += gridDim.x * blockDim.x) {
+  const int num_tiles = (total + SC_THREADS - 1) / SC_THREADS;
+  __shared__ int s_warp[SC_THREADS / 32];
+  __shared__ int s_tile, s_prefix;
+  while (true) {
+    if (threadIdx.x == 0) s_tile = (int)atomicAdd(counter, 1u);
+    __syncthreads();
+    const int tile = s_tile;
+    if (tile >= num_tiles) {
+      if (threadIdx.x == 0) dispenser_exit<false>(counter);
+      return;
+    }
+    const int f = tile * SC_THREADS + threadIdx.x;
     const int lv = (f >= a.start[2]) ? 2 : (f >= a.start[1] ? 1 : 0);
     const int rows = a.rows[lv], cols = a.cols[lv];
     const int p = f - a.start[lv];
     const uint8_t* __restrict__ src = a.src[lv];
     const int y = p / cols, x = p - y * cols;
-    float dxVal = 0, dyVal = 0;
-    int kernelIndex = 8;
-    for (int j = max(y - 1, 0); j <= min(y + 1, rows - 1); j++)
-      for (int i = max(x - 1, 0); i <= min(x + 1, cols - 1); i++) {
-        const float s = (float)src[(size_t)j * cols + i];
-        dxVal += s * gsx[kernelIndex];
-        dyVal += s * gsy[kernelIndex];
-        --kernelIndex;
+    int valx = 0, valy = 0;
+    bool ok = false;
+    if (f < total) {
+      float dxVal = 0, dyVal = 0;
+      int kernelIndex = 8;
+      for (int j = max(y - 1, 0); j <= min(y + 1, rows - 1); j++)
+        for (int i = max(x - 1, 0); i <= min(x + 1, cols - 1); i++) {
+          const float s = (float)src[(size_t)j * cols + i];
+          dxVal += s * gsx[kernelIndex];
+          dyVal += s * gsy[kernelIndex];
+          --kernelIndex;
+        }
+      valx = (int16_t)__float2int_rz(dxVal);
+      valy = (int16_t)__float2int_rz(dyVal);
+      a.dx[lv][p] = (int16_t)valx;
+      a.dy[lv][p] = (int16_t)valy;
+      ok = (x < cols - 5 && y < rows - 1);
+      if (ok) {
+        const float mTwo = (float)((valx * valx) + (valy * valy));
+        ok = (mTwo >= a.minScale[lv]) && !isnan(a.depth[lv][p]);
       }
-    const int valx = (int16_t)__float2int_rz(dxVal), valy = (int16_t)__float2int_rz(dyVal);
-    a.dx[lv][p] = (int16_t)valx;
-    a.dy[lv][p] = (int16_t)valy;
-    bool ok = (x < cols - 5 && y < rows - 1);
-    if (ok) {
-      const float mTwo = (float)((valx * valx) + (valy * valy));
-      ok = (mTwo >= a.minScale[lv]) && !isnan(a.depth[lv][p]);
+      if (ok) {
+        for (int u = max(y - 2, 0); u < min(y + 2, rows); u++)
+          for (int v = max(x - 2, 0); v < min(x + 2, cols); v++) ok = ok && (src[(size_t)u * cols + v] > 0);
+      }
     }
-    if (ok) {
-      for (int u = max(y - 2, 0); u < min(y + 2, rows); u++)
-        for (int v = max(x - 2, 0); v < min(x + 2, cols); v++) ok = ok && (src[(size_t)u * cols + v] > 0);
+    int aggregate;
+    const int excl = block_exclusive_scan<SC_THREADS>(ok ? 1 : 0, s_warp, aggregate);
+    if (threadIdx.x < 32) {
+      const int prefix = lookback_prefix(state, tile, 0, 0, aggregate, epoch);
+      if (threadIdx.x == 0) {
+        s_prefix = prefix;
+        if (tile == num_tiles - 1) gn->cand_base[NUM_PYRS] = prefix + aggregate;
+      }
     }
-    flags[f] = ok ? 1 : 0;
-  }
-}
-
-__global__ void k_cand_scatter(SobelArgs a, const uint8_t* __restrict__ flags, const int* __restrict__ offsets, int4* __restrict__ cand,
-                               GNState* gn) {
-  pdl_enter();
-  const int total = a.start[NUM_PYRS];
-  for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < total; f += gridDim.x * blockDim.x) {
-    const int lv = (f >= a.start[2]) ? 2 : (f >= a.start[1] ? 1 : 0);
-    const int o = offsets[f];
-    if (f == a.start[lv]) gn->cand_base[lv] = o;  // exclusive prefix at the first pixel of the level
-    if (!flags[f]) continue;
-    const int p = f - a.start[lv];
-    const int g = ((int)(uint16_t)a.dx[lv][p]) | (((int)(uint16_t)a.dy[lv][p]) << 16);
-    cand[o] = make_int4(p, __float_as_int(a.depth[lv][p]), g, (int)a.src[lv][p]);
+    __syncthreads();
+    const int o = s_prefix + excl;
+    if (f < total && f == a.start[lv]) gn->cand_base[lv] = o;  // exclusive prefix at the first pixel of the level
+    if (ok) {
+      const int g = ((int)(uint16_t)valx) | (((int)(uint16_t)valy) << 16);
+      cand[o] = make_int4(p, __float_as_int(a.depth[lv][p]), g, (int)src[p]);
+    }
+    __syncthreads();  // s_tile and s_prefix are rewritten by the next draw
   }
 }
 
@@ -555,7 +577,7 @@ int map_select_model_inputs(EfContext* ctx) {
   Textures& t = ctx->tex;
   const size_t n = (size_t)od.width * od.height;
   EF_LAUNCH(ctx, k_model_level0, wave_blocks(ctx, n), 256, 0, (const float4*)t.vertex, (const float4*)t.normal, (const float4*)t.fill_vertex,
-            (const float4*)t.fill_normal, (const uchar4*)t.image, (const uchar4*)t.fill_image, (const int*)ctx->map.dense_flag,
+            (const float4*)t.fill_normal, (const uchar4*)t.image, (const uchar4*)t.fill_image, (const int*)ctx->map.dense_count,
             ctx->frame_to_frame_rgb ? 1 : 0, od.height, od.width, od.maxDepthRGB, (float4*)od.vmaps_tmp, od.vmap_c_prev[0], od.nmap_c_prev[0],
             od.lastDepth[0], od.lastImage[0]);
   for (int i = 0; i + 1 < NUM_PYRS; ++i)
@@ -580,13 +602,10 @@ int launch_sobel(EfContext* ctx, int which) {
     a.minScale[i] = od.minScale[i];
   }
   a.start[NUM_PYRS] = od.level_start[NUM_PYRS];
-  const size_t flat = (size_t)od.level_start[NUM_PYRS];
-  uint8_t* flags;
-  int* offsets;
-  scan_scratch(ctx, &flags, &offsets);
-  EF_LAUNCH(ctx, k_sobel_cand, wave_blocks(ctx, flat), 256, 0, a, flags);
-  RC(run_scan(ctx, flags, &od.gn->flat_n, nullptr, flat, offsets, &od.gn->cand_base[NUM_PYRS]));
-  EF_LAUNCH(ctx, k_cand_scatter, wave_blocks(ctx, flat), 256, 0, a, (const uint8_t*)flags, (const int*)offsets, od.cand, od.gn);
+  ScanSlot sc;
+  RC(scan_slot(ctx, &sc));
+  EF_LAUNCH(ctx, k_sobel_cand, wave_blocks(ctx, (size_t)od.level_start[NUM_PYRS], 8, SC_THREADS), SC_THREADS, 0, a, od.cand, od.gn, sc.state,
+            sc.counter, sc.epoch);
   ctx->maps_dirty[which] = true;  // k_iter1 / k_iter2 read the list ahead of their dependency wait: fence before the next one
   CHECK_LAST();
   return 0;
