@@ -50,11 +50,14 @@ __device__ __forceinline__ float gmin(float x, float y) { return (y < x) ? y : x
 __device__ __forceinline__ float gmax(float x, float y) { return (x < y) ? y : x; }  // GLSL max
 
 // 4x4 row-major float pose applied to a point / a direction, accumulation order ((m0*x + m1*y) + m2*z) + m3
-__device__ __forceinline__ f3 xform(const float* m, const f3& v) {
+// (M: any pointer to float, e.g. a volatile one into shared memory that the compiler must not hold in registers)
+template <typename M>
+__device__ __forceinline__ f3 xform(M m, const f3& v) {
   return mk3(((m[0] * v.x + m[1] * v.y) + m[2] * v.z) + m[3], ((m[4] * v.x + m[5] * v.y) + m[6] * v.z) + m[7],
              ((m[8] * v.x + m[9] * v.y) + m[10] * v.z) + m[11]);
 }
-__device__ __forceinline__ f3 rot(const float* m, const f3& v) {
+template <typename M>
+__device__ __forceinline__ f3 rot(M m, const f3& v) {
   return mk3((m[0] * v.x + m[1] * v.y) + m[2] * v.z, (m[4] * v.x + m[5] * v.y) + m[6] * v.z,
              (m[8] * v.x + m[9] * v.y) + m[10] * v.z);
 }

@@ -151,7 +151,8 @@ struct MapDev {
   uint32_t* assoc_id;     // W*H: matched surfel id (or 0xffffffff none / 0xfffffffe new)
   uint32_t* pending;      // capacity: lowest draw index that chose this surfel (0xffffffff idle)
   // z-buffers
-  unsigned long long* zbuf;  // W*H
+  unsigned long long* zbuf;        // W*H: the raycast's (k_splat_scatter / k_splat_resolve)
+  unsigned long long* index_keys;  // W*H: the index map's tagged keys (IndexMap in ef_map.cu)
   // scan scratch
   int* scan_tile_state;   // decoupled look-back
   unsigned int* scan_counter;
@@ -267,13 +268,15 @@ struct EfContext {
   cudaEvent_t stage_ev[16];
   int stage_n;
   bool pdl;  // programmatic dependent launch on every kernel (default on; EF_NO_PDL=1 disables)
-  bool vis_pending;      // the first pass of a frame has filled the visible list and the second has not consumed it yet
+  bool vis_pending;      // the first pass of a frame has filled the visible list and no clean has re-armed it yet
   bool visible_list;      // second index-map pass of a frame visits only the surfels the first one rasterised; EF_VISIBLE_LIST=0 disables
   int gn_cluster;         // CTAs of the clusters that run the SO(3) loop and the coarse-level Gauss-Newton iterations (0: plain launches everywhere)
   int gn_cluster_levels;  // pyramid levels, from the coarsest, whose iterations run in that cluster
   bool la_after_track;    // the look-ahead's side stream starts after the frame's coarse-level cluster (EF_LA_AFTER_TRACK=0: at frame start)
   bool plain_next;     // the next ef_launch omits the programmatic-serialisation attribute (EF_PLAIN_NEXT)
   bool maps_dirty[2];  // a kernel that writes tracker w's pyramids may still be in flight ahead of the next stage launch
+  int index_pass;      // index-map passes since MapDev::index_keys was last re-armed: the current pass's tag is 0xff - index_pass
+  bool index_keys_only;  // the last index pass was a frame's: fuse and clean read its keys, the frame's clean writes its textures
 
   ef::OdomDev odom[2];
   ef::MapDev map;
@@ -417,6 +420,8 @@ int scan_slot(EfContext* ctx, ScanSlot* out);
 int map_initialise_async(EfContext* ctx);
 int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
 int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, int time_delta, int vis_mode = 0);
+// the textures of a frame's index pass that no clean has written yet (nothing to do otherwise)
+int map_index_textures_async(EfContext* ctx);
 int map_fuse_async(EfContext* ctx, int time_or_neg, float max_depth, float weighting_or_neg);
 int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0, bool is_fern = false);
 int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);

@@ -190,14 +190,70 @@ __device__ __forceinline__ WinAxis window_axis(float centre, float step, int n) 
   }
   return A;
 }
-// the index texels of the window spanned by two axes, cur[3 * x + y] (x outer, y inner, ascending); texels no sample lands
-// on read as empty (0)
-__device__ __forceinline__ void window_index(const uint32_t* index, int cols, const WinAxis& ax, const WinAxis& ay, uint32_t (&cur)[9]) {
+// The index map (index_map.vert/.frag). A pass of k_index_scatter leaves one key per texel in `keys`: [63:56] the pass's tag,
+// [55:32] window depth d24, [31:0] surfel id. Tags count down from 0xfe, one per pass, and the host re-arms the buffer (all
+// 0xff) before they run out, so a key of the current pass is smaller than every key an earlier pass left: atomicMin still picks
+// the nearest surfel, the lower id on ties, and no pass has to clear the buffer. A texel is occupied iff its key carries the
+// current tag. The textures (EF_BUF_INDEX, VERT_CONF, COLOR_TIME, NORM_RAD) are written from the keys by write_index_texels:
+// by the stage API's pass itself, and by the frame's clean for the frame's passes. Inside a frame the map does not change
+// between an index pass and its reader (fuse writes only after k_fuse_associate, clean moves surfels only after
+// k_clean_flags), so there fuse and clean read the keys and the surfels they name; otherwise (TEX) they read the textures,
+// which a stage-API caller may have uploaded or may have changed the map under.
+struct IndexMap {
+  const unsigned long long* keys;
+  unsigned int tag;
+  uint32_t* index;
+  float4 *vert_conf, *col_time, *norm_rad;
+};
+__device__ __forceinline__ bool key_live(unsigned long long key, unsigned int tag) { return (unsigned int)(key >> 56) == tag; }
+// texel attributes of a surfel: camera-space vertex + confidence, camera-space unit normal + radius (colour + time is copied)
+template <typename M>
+__device__ __forceinline__ float4 index_vert_conf(M t_inv, const float4& pc) {
+  const f3 h = xform(t_inv, mk3(pc.x, pc.y, pc.z));
+  return make_float4(h.x, h.y, h.z, pc.w);
+}
+__device__ __forceinline__ float4 index_norm_rad(const float* t_inv, const float4& nr) {
+  const f3 nn = normalized(rot(t_inv, mk3(nr.x, nr.y, nr.z)));
+  return make_float4(nn.x, nn.y, nn.z, nr.w);
+}
+// the textures of texels first, first + stride, ... < n_px; an empty texel is all zeros
+__device__ __forceinline__ void write_index_texels(const IndexMap& ix, const MapPose* __restrict__ mp, const float4* __restrict__ pos_conf,
+                                                   const float4* __restrict__ color_time, const float4* __restrict__ norm_rad, int n_px,
+                                                   int first, int stride) {
+  for (int p = first; p < n_px; p += stride) {
+    const unsigned long long key = ix.keys[p];
+    if (!key_live(key, ix.tag)) {
+      ix.index[p] = 0;
+      ix.vert_conf[p] = ix.col_time[p] = ix.norm_rad[p] = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
+    const uint32_t id = (uint32_t)key;
+    const float4 pc = pos_conf[id], nr = norm_rad[id];
+    ix.index[p] = id;
+    ix.vert_conf[p] = index_vert_conf(mp->t_inv, pc);
+    ix.col_time[p] = color_time[id];
+    ix.norm_rad[p] = index_norm_rad(mp->t_inv, nr);
+  }
+}
+// the surfel ids of the window spanned by two axes, cur[3 * x + y] (x outer, y inner, ascending); texels no sample lands on,
+// and empty texels, read as 0 (as in the reference, surfel 0 is never a match)
+template <bool TEX>
+__device__ __forceinline__ void window_index(const IndexMap& ix, int cols, const WinAxis& ax, const WinAxis& ay, uint32_t (&cur)[9]) {
 #pragma unroll
   for (int ia = 0; ia < 3; ++ia)
 #pragma unroll
-    for (int jb = 0; jb < 3; ++jb)
-      cur[ia * 3 + jb] = (ax.m[ia] > 0 && ay.m[jb] > 0) ? index[(ay.t0 + jb) * cols + (ax.t0 + ia)] : 0u;
+    for (int jb = 0; jb < 3; ++jb) {
+      cur[ia * 3 + jb] = 0u;
+      if (ax.m[ia] > 0 && ay.m[jb] > 0) {
+        const int p = (ay.t0 + jb) * cols + (ax.t0 + ia);
+        if (TEX) {
+          cur[ia * 3 + jb] = ix.index[p];
+        } else {
+          const unsigned long long key = ix.keys[p];
+          cur[ia * 3 + jb] = key_live(key, ix.tag) ? (uint32_t)key : 0u;
+        }
+      }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -328,8 +384,9 @@ __global__ void k_init_scatter(const uint8_t* __restrict__ rgb, const float* __r
 template <int MODE>
 __global__ void __launch_bounds__(256, 5) k_index_scatter(const float4* __restrict__ pos_conf, const float4* __restrict__ color_time,
                                                           const int* __restrict__ count, const MapPose* __restrict__ mp, int time, float max_depth,
-                                                          int time_delta, int rows, int cols, Cam c, unsigned long long* __restrict__ zbuf,
-                                                          uint32_t* __restrict__ vis, int* __restrict__ vis_count, int vis_capacity) {
+                                                          int time_delta, int rows, int cols, Cam c, unsigned long long* __restrict__ keys,
+                                                          unsigned int tag, uint32_t* __restrict__ vis, int* __restrict__ vis_count,
+                                                          int vis_capacity) {
   pdl_enter();
   const int n_map = *count;
   const int n = (MODE == 2) ? min(*vis_count, vis_capacity) : n_map;
@@ -374,8 +431,8 @@ __global__ void __launch_bounds__(256, 5) k_index_scatter(const float4* __restri
       if (px < 0 || py < 0 || px >= cols || py >= rows) continue;
       const unsigned int d24 = depth24(0.5f * zn + 0.5f);
       if (d24 >= 16777215u) continue;
-      key[u] = ((unsigned long long)d24 << 32) | (unsigned int)id;
-      slot[u] = &zbuf[(size_t)py * cols + px];
+      key[u] = ((unsigned long long)tag << 56) | ((unsigned long long)d24 << 32) | (unsigned int)id;
+      slot[u] = &keys[(size_t)py * cols + px];
       cur[u] = __ldcg(slot[u]);
     }
 #pragma unroll
@@ -404,30 +461,11 @@ __global__ void __launch_bounds__(256, 5) k_index_scatter(const float4* __restri
   }
 }
 
-__global__ void k_index_resolve(const float4* __restrict__ pos_conf, const float4* __restrict__ color_time, const float4* __restrict__ norm_rad,
-                                const MapPose* __restrict__ mp, int n_px, unsigned long long* __restrict__ zbuf,
-                                uint32_t* __restrict__ index, float4* __restrict__ vert_conf, float4* __restrict__ col_time,
-                                float4* __restrict__ nrm_rad, int* __restrict__ reset_count) {
+// the textures of the last index pass, for a caller of the stage API (the frame's second pass has k_clean_flags write them)
+__global__ void k_index_textures(IndexMap ix, const float4* __restrict__ pos_conf, const float4* __restrict__ color_time,
+                                 const float4* __restrict__ norm_rad, const MapPose* __restrict__ mp, int n_px) {
   pdl_enter();
-  if (reset_count && blockIdx.x == 0 && threadIdx.x == 0) *reset_count = 0;  // the visible list has been consumed: re-arm it
-  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n_px; p += gridDim.x * blockDim.x) {
-    const unsigned long long key = zbuf[p];
-    zbuf[p] = kEmptyKey;  // the resolve pass leaves the z-buffer cleared for the next scatter (no memset between passes)
-    if (key == kEmptyKey) {
-      index[p] = 0;
-      vert_conf[p] = col_time[p] = nrm_rad[p] = make_float4(0.f, 0.f, 0.f, 0.f);
-      continue;
-    }
-    const uint32_t id = (uint32_t)(key & 0xffffffffull);
-    const float4 pc = pos_conf[id];
-    const float4 nr = norm_rad[id];
-    const f3 h = xform(mp->t_inv, mk3(pc.x, pc.y, pc.z));
-    const f3 nn = normalized(rot(mp->t_inv, mk3(nr.x, nr.y, nr.z)));
-    index[p] = id;
-    vert_conf[p] = make_float4(h.x, h.y, h.z, pc.w);
-    col_time[p] = color_time[id];
-    nrm_rad[p] = make_float4(nn.x, nn.y, nn.z, nr.w);
-  }
+  write_index_texels(ix, mp, pos_conf, color_time, norm_rad, n_px, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -437,9 +475,7 @@ struct FuseArgs {
   const uint8_t* rgb;
   const float* depth_raw;
   const float* depth_filt;
-  const uint32_t* index;
-  const float4* vert_conf;
-  const float4* norm_rad;
+  IndexMap ix;  // (read only)
   int rows, cols;
   Cam c;
   int time;
@@ -474,7 +510,10 @@ __device__ __forceinline__ bool fuse_active(const FuseArgs& a, int i, int j, Pix
 
 constexpr uint32_t ASSOC_NONE = 0xffffffffu, ASSOC_NEW = 0xfffffffeu;
 
-__global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint32_t* __restrict__ assoc, uint32_t* __restrict__ pending) {
+template <bool TEX>
+__global__ void k_fuse_associate(FuseArgs a, const MapPose* __restrict__ mp, const float4* __restrict__ pos_conf,
+                                 const float4* __restrict__ norm_rad, const int* __restrict__ count, uint32_t* __restrict__ assoc,
+                                 uint32_t* __restrict__ pending) {
   pdl_enter();
   const Quarter Q = quarter_of(a.time, a.rows, a.cols);
   const int nq = Q.ni * Q.nj;
@@ -504,16 +543,24 @@ __global__ void k_fuse_associate(FuseArgs a, const int* __restrict__ count, uint
       // of the occupied ones column by column: four dependent memory round trips instead of one or two per texel.
       const WinAxis ax = window_axis(g.tcx, indexXStep, a.cols), ay = window_axis(g.tcy, indexYStep, a.rows);
       uint32_t cur[9];
-      window_index(a.index, a.cols, ax, ay, cur);
+      window_index<TEX>(a.ix, a.cols, ax, ay, cur);
 #pragma unroll
       for (int ia = 0; ia < 3; ++ia) {
         float4 vc[3], nr[3];
 #pragma unroll
-        for (int jb = 0; jb < 3; ++jb)
-          if (cur[ia * 3 + jb] > 0U) {
+        for (int jb = 0; jb < 3; ++jb) {
+          const uint32_t id = cur[ia * 3 + jb];
+          if (id > 0U) {
             const int p = (ay.t0 + jb) * a.cols + (ax.t0 + ia);
-            vc[jb] = a.vert_conf[p];
-            nr[jb] = a.norm_rad[p];
+            vc[jb] = TEX ? a.ix.vert_conf[p] : pos_conf[id];
+            nr[jb] = TEX ? a.ix.norm_rad[p] : norm_rad[id];
+          }
+        }
+#pragma unroll
+        for (int jb = 0; jb < 3; ++jb)
+          if (!TEX && cur[ia * 3 + jb] > 0U) {
+            vc[jb] = index_vert_conf(mp->t_inv, vc[jb]);
+            nr[jb] = index_norm_rad(mp->t_inv, nr[jb]);
           }
 #pragma unroll
         for (int jb = 0; jb < 3; ++jb) {
@@ -645,9 +692,7 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_update(FuseArgs a, const Ma
 // clean: copy_unstable.vert/.geom without deformation graph (GlobalModel.cpp:527-671)
 // ---------------------------------------------------------------------------------------------------------------
 struct CleanArgs {
-  const uint32_t* index;
-  const float4* vert_conf;
-  const float4* col_time;
+  IndexMap ix;
   int rows, cols;
   Cam c;
   int time;
@@ -769,10 +814,16 @@ __device__ __noinline__ void deform_surfel(const CleanArgs& a, const MapPose* mp
   }
 }
 
-__device__ __forceinline__ bool clean_test(const CleanArgs& a, const MapPose* mp, const float4& pos, float4& col, const float4* __restrict__ nr_ptr) {
+// t_inv_s: the map pose's inverse, in shared memory. The window's surfels are transformed through a volatile view of it: the
+// pose is read from shared memory per texel instead of being held in 12 registers across the window.
+template <bool TEX>
+__device__ __forceinline__ bool clean_test(const CleanArgs& a, const float* t_inv_s, const float4* __restrict__ pos_conf,
+                                           const float4* __restrict__ color_time, const float4& pos, float4& col,
+                                           const float4* __restrict__ nr_ptr) {
   const float fcols = (float)a.cols, frows = (float)a.rows;
   int test = 1;
-  const f3 localPos = xform(mp->t_inv, mk3(pos.x, pos.y, pos.z));
+  const volatile float* t_inv_v = t_inv_s;
+  const f3 localPos = TEX ? xform(t_inv_s, mk3(pos.x, pos.y, pos.z)) : xform(t_inv_v, mk3(pos.x, pos.y, pos.z));
   const float x = ((a.c.fx * localPos.x) / localPos.z) + a.c.cx;
   const float y = ((a.c.fy * localPos.y) / localPos.z) + a.c.cy;
   const float scale = 1.0f;
@@ -781,32 +832,39 @@ __device__ __forceinline__ bool clean_test(const CleanArgs& a, const MapPose* mp
   int count = 0, zCount = 0;
   if ((float)a.time - col.w < (float)a.time_delta && localPos.z > 0 && x > 0 && y > 0 && x < fcols && y < frows) {
     const float4 nr = *nr_ptr;  // normal + radius: only the surfels in view need them (32 B instead of 48 for the rest)
-    const f3 localNorm = normalized(rot(mp->t_inv, mk3(nr.x, nr.y, nr.z)));
+    const f3 localNorm = normalized(TEX ? rot(t_inv_s, mk3(nr.x, nr.y, nr.z)) : rot(t_inv_v, mk3(nr.x, nr.y, nr.z)));
     // duplicate samples COUNT here (copy_unstable.vert:94,106; SURVEY App. A-19): each distinct texel is read once and
     // weighted by the number of float-loop samples that land on it. Index texels first, attributes of the occupied ones after.
     const WinAxis ax = window_axis(x / fcols, indexXStep, a.cols), ay = window_axis(y / frows, indexYStep, a.rows);
     uint32_t cur[9];
-    window_index(a.index, a.cols, ax, ay, cur);
+    window_index<TEX>(a.ix, a.cols, ax, ay, cur);
 #pragma unroll
     for (int ia = 0; ia < 3; ++ia) {
-      float4 vcs[3], cts[3];
+      float4 vcs[3];
+      float2 its[3];  // (init time, last time): the colour half is not read
+#pragma unroll
+      for (int jb = 0; jb < 3; ++jb) {
+        const uint32_t id = cur[ia * 3 + jb];
+        if (id > 0U) {
+          const int p = (ay.t0 + jb) * a.cols + (ax.t0 + ia);
+          vcs[jb] = TEX ? a.ix.vert_conf[p] : pos_conf[id];
+          its[jb] = reinterpret_cast<const float2*>(TEX ? a.ix.col_time + p : color_time + id)[1];
+        }
+      }
 #pragma unroll
       for (int jb = 0; jb < 3; ++jb)
-        if (cur[ia * 3 + jb] > 0U) {
-          const int p = (ay.t0 + jb) * a.cols + (ax.t0 + ia);
-          vcs[jb] = a.vert_conf[p];
-          cts[jb] = a.col_time[p];
-        }
+        if (!TEX && cur[ia * 3 + jb] > 0U) vcs[jb] = index_vert_conf(t_inv_v, vcs[jb]);
 #pragma unroll
       for (int jb = 0; jb < 3; ++jb)
         if (cur[ia * 3 + jb] > 0U) {
           const int m = ax.m[ia] * ay.m[jb];
-          const float4 vc = vcs[jb], ct = cts[jb];
+          const float4 vc = vcs[jb];
+          const float2 it = its[jb];
           const float dx = vc.x - localPos.x, dy = vc.y - localPos.y;
-          if (ct.z < col.z && vc.w > a.conf_threshold && vc.z > localPos.z && vc.z - localPos.z < 0.01f &&
+          if (it.x < col.z && vc.w > a.conf_threshold && vc.z > localPos.z && vc.z - localPos.z < 0.01f &&
               sqrtf(dx * dx + dy * dy) < nr.w * 1.4f)
             count += m;
-          if (ct.w == (float)a.time && vc.w > a.conf_threshold && vc.z > localPos.z && vc.z - localPos.z > 0.01f &&
+          if (it.y == (float)a.time && vc.w > a.conf_threshold && vc.z > localPos.z && vc.z - localPos.z > 0.01f &&
               fabsf(localNorm.z) > 0.85f)
             zCount += m;
         }
@@ -821,6 +879,12 @@ __device__ __forceinline__ bool clean_test(const CleanArgs& a, const MapPose* mp
 
 // ---- TMA-style 1-D bulk copies (cp.async.bulk, SASS UBLKCP) + mbarrier, used to stage surfel tiles in shared memory ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// global -> shared copy of 8 or 16 bytes that holds no register while in flight (cp.async, completed by cp_async_wait)
+template <int BYTES>
+__device__ __forceinline__ void cp_async(void* dst_smem, const void* src_gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "n"(BYTES) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -876,27 +940,36 @@ constexpr int CC_WORDS = CC_ITEMS * (CC_THREADS / 32);  // keep-mask words per t
 // ctl[0] tile dispenser, ctl[1] exit tickets, ctl[2] first tile that moves (0xffffffff: none)
 constexpr int CF_THREADS = CC_TILE;  // one surfel per thread: the window test is a chain of ~5 dependent gathers, so two surfels per
                                      // thread would double the latency of a small map's pass (27 -> 14 us at 270 k surfels)
+// write_tex: the index textures are still to be written from the keys (the frame's passes leave that to this kernel, which
+// runs before k_clean_move moves a surfel); reset_count: the visible list the frame's index passes used, re-armed here
+template <bool TEX>
 __global__ void __launch_bounds__(CF_THREADS, 2) k_clean_flags(CleanArgs a, const MapPose* __restrict__ mp, const float4* __restrict__ pos_conf,
                                                                const float4* __restrict__ color_time, const float4* __restrict__ norm_rad,
                                                                const int* __restrict__ count, const float4* __restrict__ new_pos,
                                                                const float4* __restrict__ new_col, const float4* __restrict__ new_nr,
                                                                const int* __restrict__ new_count, uint32_t* __restrict__ keep_mask,
-                                                               unsigned int* ctl) {
+                                                               unsigned int* ctl, int write_tex, int* __restrict__ reset_count) {
   pdl_enter();
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  if (reset_count && blockIdx.x == 0 && tid == 0) *reset_count = 0;
+  __shared__ float s_tinv[16];
+  if (!TEX && tid < 16) s_tinv[tid] = mp->t_inv[tid];
+  __syncthreads();
   const int n_old = *count, total = n_old + *new_count;
   const int num_tiles = (total + CC_TILE - 1) / CC_TILE;
-  // (the next tile's position / colour-time records are requested before this tile is tested: two rounds in flight)
-  auto fetch = [&](int t, float4& pos, float4& col) {
+  // The next tile's position and (init time, last time) are requested before this tile is tested: two rounds in flight. They
+  // are staged in this thread's own shared-memory slot by cp.async, so they hold no registers across the test.
+  __shared__ float4 s_pos[CF_THREADS];
+  __shared__ float2 s_time[CF_THREADS];
+  auto fetch = [&](int t) {
     const int g = t * CC_TILE + tid;
     if (t < num_tiles && g < total) {
       const bool is_old = g < n_old;
-      pos = is_old ? pos_conf[g] : new_pos[g - n_old];
-      col = is_old ? color_time[g] : new_col[g - n_old];
+      cp_async<16>(&s_pos[tid], is_old ? pos_conf + g : new_pos + (g - n_old));
+      cp_async<8>(&s_time[tid], reinterpret_cast<const float2*>(is_old ? color_time + g : new_col + (g - n_old)) + 1);
     }
   };
-  float4 pos_next = make_float4(0.f, 0.f, 0.f, 0.f), col_next = pos_next;
-  fetch(blockIdx.x, pos_next, col_next);
+  fetch(blockIdx.x);
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
     const int g0 = t * CC_TILE;
     const int n_in = min(CC_TILE, total - g0);
@@ -904,13 +977,15 @@ __global__ void __launch_bounds__(CF_THREADS, 2) k_clean_flags(CleanArgs a, cons
     bool moves = (g0 + n_in > n_old) || a.n_nodes > 0;
     // thread = item of the tile: warp w holds items 32 w .. 32 w + 31, i.e. keep-mask word w in k_clean_move's (slab, warp) order
     const int g = g0 + tid;
-    const float4 pos = pos_next;
-    float4 col = col_next;
-    fetch(t + gridDim.x, pos_next, col_next);
+    cp_async_wait();
+    const float4 pos = s_pos[tid];
+    const float2 it = s_time[tid];
+    float4 col = make_float4(0.f, 0.f, it.x, it.y);  // (clean_test reads only the times)
+    fetch(t + gridDim.x);
     bool keep = false;
     if (tid < n_in) {
       const bool is_old = g < n_old;
-      keep = clean_test(a, mp, pos, col, is_old ? norm_rad + g : new_nr + (g - n_old));
+      keep = clean_test<TEX>(a, TEX ? mp->t_inv : s_tinv, pos_conf, color_time, pos, col, is_old ? norm_rad + g : new_nr + (g - n_old));
     }
     const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
     const unsigned int valid = __ballot_sync(0xffffffffu, tid < n_in);
@@ -918,6 +993,8 @@ __global__ void __launch_bounds__(CF_THREADS, 2) k_clean_flags(CleanArgs a, cons
     moves = moves || ballot != valid;
     if (moves && lane == 0) atomicMin(ctl + 2, (unsigned int)t);
   }
+  if (!TEX && write_tex)  // (textures that clean reads are already written)
+    write_index_texels(a.ix, mp, pos_conf, color_time, norm_rad, a.rows * a.cols, blockIdx.x * CF_THREADS + tid, gridDim.x * CF_THREADS);
 }
 
 template <bool DEFORM>
@@ -1431,7 +1508,11 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &m.new_count, 4, 0));
   CU(ctx_alloc(ctx, &m.assoc_id, n));
   CU(ctx_alloc(ctx, &m.pending, cap, 0xff));
-  CU(ctx_alloc(ctx, &m.zbuf, n, 0xff));  // kept cleared by the resolve passes from here on
+  CU(ctx_alloc(ctx, &m.zbuf, n, 0xff));  // kept cleared by k_splat_resolve from here on
+  // as if the tags had just run out: before the first pass re-arms it, no key carries the tag (0) fuse and clean look for
+  CU(ctx_alloc(ctx, &m.index_keys, n, 0xff));
+  ctx->index_pass = 255;
+  ctx->index_keys_only = false;
   // look-back tile states: the clean pass walks capacity + n surfels in tiles of CC_TILE, the image-sized compactions
   // (first-frame feedback, new surfels, the tracker's candidate list) <= 2 n items in tiles of at least 128
   const size_t max_items = cap + n;
@@ -1525,22 +1606,50 @@ int map_initialise_async(EfContext* ctx) {
   return 0;
 }
 
-// vis_mode 0: plain (stage API). 1: also record the surfels that reach the z-buffer (first pass of a frame). 2: visit only those
-// (second pass of the frame, same arguments, only fuse in between) and re-arm the list.
+static IndexMap index_map(EfContext* ctx) {
+  IndexMap ix;
+  ix.keys = ctx->map.index_keys;
+  ix.tag = 0xffu - (unsigned int)ctx->index_pass;
+  ix.index = ctx->tex.index;
+  ix.vert_conf = ctx->tex.vert_conf;
+  ix.col_time = ctx->tex.color_time;
+  ix.norm_rad = ctx->tex.norm_rad;
+  return ix;
+}
+
+// vis_mode 0: plain (stage API), textures written. 1: also record the surfels that reach the z-buffer (first pass of a frame).
+// 2: visit only those (second pass of the frame, same arguments, only fuse in between). The frame's passes (1, 2) leave the
+// textures to the frame's clean, which also re-arms the list.
 int map_predict_indices_async(EfContext* ctx, int time, float max_depth, int time_delta, int vis_mode) {
   MapDev& m = ctx->map;
   const int n = m.rows * m.cols;
+  const bool in_frame = vis_mode != 0;
   if (!ctx->visible_list) vis_mode = 0;
   const int grid = ctx->num_sms * 5;
-  if (vis_mode == 1 && ctx->vis_pending) CU(cudaMemsetAsync(m.vis_count, 0, 4, ctx->stream));  // (a frame that failed between its two passes)
+  if (vis_mode == 1 && ctx->vis_pending) CU(cudaMemsetAsync(m.vis_count, 0, 4, ctx->stream));  // (a frame that failed before its clean)
   if (vis_mode == 2 && !ctx->vis_pending) vis_mode = 0;
   if (vis_mode == 1) ctx->vis_pending = true;
-  if (vis_mode == 2) ctx->vis_pending = false;
+  if (ctx->index_pass == 255) {  // the tags have run out: every key becomes stale
+    CU(cudaMemsetAsync(m.index_keys, 0xff, (size_t)n * sizeof(unsigned long long), ctx->stream));
+    ctx->index_pass = 0;
+  }
+  ctx->index_pass++;
+  const IndexMap ix = index_map(ctx);
   const auto scatter = vis_mode == 1 ? k_index_scatter<1> : vis_mode == 2 ? k_index_scatter<2> : k_index_scatter<0>;  // (mode 0 never reads the list)
   EF_LAUNCH(ctx, scatter, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols, cam_of(ctx),
-            m.zbuf, m.vis_list, m.vis_count, m.capacity);
-  EF_LAUNCH(ctx, k_index_resolve, wave_blocks(ctx, n), 256, 0, m.pos_conf, m.color_time, m.norm_rad, m.pose, n, m.zbuf, ctx->tex.index,
-            ctx->tex.vert_conf, ctx->tex.color_time, ctx->tex.norm_rad, vis_mode == 2 ? m.vis_count : (int*)nullptr);
+            m.index_keys, ix.tag, m.vis_list, m.vis_count, m.capacity);
+  ctx->index_keys_only = in_frame;
+  if (!in_frame) EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, ix, m.pos_conf, m.color_time, m.norm_rad, m.pose, n);
+  CHECK_LAST();
+  return 0;
+}
+
+int map_index_textures_async(EfContext* ctx) {
+  if (!ctx->index_keys_only) return 0;
+  MapDev& m = ctx->map;
+  const int n = m.rows * m.cols;
+  EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, index_map(ctx), m.pos_conf, m.color_time, m.norm_rad, m.pose, n);
+  ctx->index_keys_only = false;
   CHECK_LAST();
   return 0;
 }
@@ -1550,9 +1659,7 @@ static FuseArgs fuse_args(EfContext* ctx, int time, float max_depth) {
   a.rgb = ctx->tex.rgb;
   a.depth_raw = ctx->tex.depth_metric;
   a.depth_filt = ctx->tex.depth_metric_filtered;
-  a.index = ctx->tex.index;
-  a.vert_conf = ctx->tex.vert_conf;
-  a.norm_rad = ctx->tex.norm_rad;
+  a.ix = index_map(ctx);
   a.rows = ctx->map.rows;
   a.cols = ctx->map.cols;
   a.c = cam_of(ctx);
@@ -1572,7 +1679,8 @@ int map_fuse_async(EfContext* ctx, int time, float max_depth, float weighting) {
   FuseArgs a = fuse_args(ctx, time, max_depth);
   const Quarter Q = quarter_of(time, m.rows, m.cols);
   const int nq = Q.ni * Q.nj;
-  EF_LAUNCH(ctx, k_fuse_associate, wave_blocks(ctx, nq, 16, 128), 128, 0, a, m.count, m.assoc_id, m.pending);
+  const auto associate = ctx->index_keys_only ? k_fuse_associate<false> : k_fuse_associate<true>;
+  EF_LAUNCH(ctx, associate, wave_blocks(ctx, nq, 16, 128), 128, 0, a, m.pose, m.pos_conf, m.norm_rad, m.count, m.assoc_id, m.pending);
   ScanSlot sc;
   RC(scan_slot(ctx, &sc));
   EF_LAUNCH(ctx, k_fuse_update, wave_blocks(ctx, nq, 16, FU_THREADS), FU_THREADS, 0, a, m.pose, (const GNState*)ctx->odom[0].gn, m.count, m.assoc_id,
@@ -1586,9 +1694,7 @@ int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_del
   MapDev& m = ctx->map;
   MapBuffers& B = mb(ctx);
   CleanArgs a;
-  a.index = ctx->tex.index;
-  a.vert_conf = ctx->tex.vert_conf;
-  a.col_time = ctx->tex.color_time;
+  a.ix = index_map(ctx);
   a.rows = m.rows;
   a.cols = m.cols;
   a.c = cam_of(ctx);
@@ -1606,8 +1712,13 @@ int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_del
   RC(next_scan_epoch(ctx, B));
   // grids never depend on a surfel count the host would have to read back: the test strides over the tiles, the movers draw
   // tiles from a dispenser (one resident wave: four 49 KB CTAs per SM)
-  EF_LAUNCH(ctx, k_clean_flags, wave_blocks(ctx, tiles, 2, 1), CF_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
-            m.new_col, m.new_nr, m.new_count, m.keep_mask, m.clean_ctl);
+  const int write_tex = ctx->index_keys_only ? 1 : 0;
+  int* reset_count = ctx->vis_pending ? m.vis_count : nullptr;
+  const auto flags = ctx->index_keys_only ? k_clean_flags<false> : k_clean_flags<true>;
+  EF_LAUNCH(ctx, flags, wave_blocks(ctx, tiles, 2, 1), CF_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
+            m.new_col, m.new_nr, m.new_count, m.keep_mask, m.clean_ctl, write_tex, reset_count);
+  ctx->index_keys_only = false;
+  ctx->vis_pending = false;
   const auto move = n_nodes > 0 ? k_clean_move<true> : k_clean_move<false>;
   EF_LAUNCH(ctx, move, wave_blocks(ctx, tiles, 4, 1), CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count,
             m.new_pos, m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
