@@ -44,6 +44,28 @@ class EfLocalDeform(C.Structure):
                 ("last_deform_time", C.c_int32), ("n_nodes", C.c_int32)]
 
 
+class EfRenderView(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("mvp", C.c_float * 16), ("mv", C.c_float * 16), ("threshold", C.c_float),
+                ("color_type", C.c_int32), ("unstable", C.c_int32), ("draw_window", C.c_int32), ("time", C.c_int32),
+                ("time_delta", C.c_int32), ("phong", C.c_int32), ("sign_mult", C.c_float)]
+
+
+def camera_view(T_wc, fx, fy, cx, cy, w, h, near=0.1, far=1000.0, **flags) -> EfRenderView:
+    """EfRenderView of a pinhole camera at pose T_wc (4x4 camera-to-world) through ef_render_camera: window pixel (i, j) samples the
+    ray through image pixel centre (i + 0.5, j + 0.5), so a render from the tracked pose with the frame's intrinsics lines up with the
+    input image, top row first. flags: threshold, color_type, unstable, draw_window, time, time_delta, phong, sign_mult (defaults:
+    the confidence threshold 10, colour type 2, sign_mult -1, the rest 0)."""
+    v = EfRenderView()
+    v.width, v.height = int(w), int(h)
+    v.threshold, v.color_type, v.sign_mult = 10.0, 2, -1.0
+    _chk(lib().ef_render_camera(_p(_T(T_wc)), _f(fx), _f(fy), _f(cx), _f(cy), int(w), int(h), _f(near), _f(far), v.mvp, v.mv))
+    for k, val in flags.items():
+        if k in ("width", "height", "mvp", "mv") or not hasattr(v, k):
+            raise KeyError(k)
+        setattr(v, k, val)
+    return v
+
+
 TRACE_DTYPE = np.dtype([
     ("kind", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("rgb_count", "<i4"), ("rgb_sigma", "<i4"),
     ("sigma_val", "<f4"),
@@ -441,6 +463,16 @@ class Context:
         out = (C.c_float * 2)()
         n = lib().ef_debug_lookahead_ms(self.h_ctx, out)
         return (out[0], out[1]) if n == 2 else None
+
+    def render(self, view: EfRenderView):
+        """ef_render_map: the map drawn as the reference viewer draws it, (H, W, 4) uint8, row 0 = window y 0."""
+        out = np.zeros((view.height, view.width, 4), np.uint8)
+        _chk(lib().ef_render_map(self.h_ctx, C.byref(view), _p(out)))
+        return out
+
+    def render_device(self, view: EfRenderView, ptr):
+        """ef_render_map_device: the same into device memory at ptr (H*W*4 bytes), asynchronous on the context's stream."""
+        _chk(lib().ef_render_map_device(self.h_ctx, C.byref(view), C.c_void_p(ptr)))
 
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)

@@ -315,6 +315,7 @@ extern "C" int ef_destroy(EfContext* ctx) {
   if (ctx->la.pin_depth) cudaFreeHost(ctx->la.pin_depth);
   map_free_host(ctx);
   deform_free(ctx);
+  render_free(ctx);
   ctx->arena.release();
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
@@ -735,6 +736,61 @@ extern "C" int ef_map_upload_range(EfContext* ctx, const float* in12, int32_t fi
 extern "C" int ef_map_upload(EfContext* ctx, const float* in12, int32_t count) {
   if (!ctx || (!in12 && count > 0) || count < 0) return EF_EINVAL;
   return map_upload(ctx, in12, count);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// global-surface render (ef_render.cu)
+// ---------------------------------------------------------------------------------------------------------------
+static bool finite_all(const float* a, int n) {
+  for (int i = 0; i < n; ++i)
+    if (!isfinite(a[i])) return false;
+  return true;
+}
+static bool render_view_ok(const EfRenderView* v) {
+  return v && v->width >= 1 && v->width <= 16384 && v->height >= 1 && v->height <= 16384 && v->color_type >= 0 && v->color_type <= 3 &&
+         finite_all(v->mvp, 16) && (!v->phong || finite_all(v->mv, 16));
+}
+extern "C" int ef_render_map_device(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_dev) {
+  if (!ctx || !rgba_dev || !render_view_ok(view)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  return render_map_async(ctx, view, rgba_dev);
+}
+extern "C" int ef_render_map(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_host) {
+  if (!ctx || !rgba_host || !render_view_ok(view)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  RC(render_map_async(ctx, view, nullptr));
+  CU(cudaMemcpyAsync(rgba_host, render_image(ctx), (size_t)view->width * view->height * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+extern "C" int ef_render_camera(const double* T_wc16, float fx, float fy, float cx, float cy, int32_t width, int32_t height, float z_near,
+                                float z_far, float* mvp16, float* mv16) {
+  if (!T_wc16 || !mvp16 || !mv16 || width < 1 || width > 16384 || height < 1 || height > 16384) return EF_EINVAL;
+  for (int i = 0; i < 16; ++i)
+    if (!isfinite(T_wc16[i])) return EF_EINVAL;
+  if (!isfinite(fx) || !isfinite(fy) || !isfinite(cx) || !isfinite(cy) || fx == 0.f || fy == 0.f || !isfinite(z_near) || !isfinite(z_far) ||
+      !(z_near > 0.f) || !(z_far > z_near))
+    return EF_EINVAL;
+  // mv = T_wc^-1 (rigid), row-major
+  double mv[16] = {0};
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) mv[r * 4 + c] = T_wc16[c * 4 + r];
+    mv[r * 4 + 3] = -(T_wc16[0 * 4 + r] * T_wc16[3] + T_wc16[1 * 4 + r] * T_wc16[7] + T_wc16[2 * 4 + r] * T_wc16[11]);
+  }
+  mv[15] = 1.0;
+  // camera looks down +z; window x = fx x/z + cx, window y = fy y/z + cy (the image's own rows: window row j is image row j), so
+  // window pixel (i, j) samples the ray through image pixel centre (i + 0.5, j + 0.5); depth -1 at z_near, +1 at z_far
+  const double W = width, H = height, n = z_near, f = z_far;
+  const double P[16] = {2.0 * fx / W, 0, 2.0 * cx / W - 1.0, 0, 0, 2.0 * fy / H, 2.0 * cy / H - 1.0, 0,
+                        0, 0, (f + n) / (f - n), -2.0 * f * n / (f - n), 0, 0, 1, 0};
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) {
+      double acc = 0;
+      for (int k = 0; k < 4; ++k) acc += P[r * 4 + k] * mv[k * 4 + c];
+      mvp16[c * 4 + r] = (float)acc;  // column-major
+      mv16[c * 4 + r] = (float)mv[r * 4 + c];
+    }
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -305,6 +305,7 @@ struct EfContext {
   ef::DevStaging* dev_small;  // device side of the per-call parameters
   void* map_host;    // host-side bookkeeping of the surfel buffers (ef_map.cu)
   void* deform;      // workspace of the deformation-graph solve (ef_deform.cu), allocated by its first call
+  void* render;      // z-buffer and image of ef_render_map* (ef_render.cu), allocated by the first render and grown with the view
   ef::Arena arena;   // every device buffer of the context
 };
 
@@ -446,4 +447,9 @@ int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_ti
 int deform_solve_local(EfContext* ctx, const float4* graph, int n, const double* src3, const double* dst3, const int* dst_times, int n_cons,
                        bool pin, int src_time, int last_deform_time, EfDeformResult* out, const float** nodes16_dev);
 void deform_free(EfContext* ctx);
+
+// ef_render.cu: the global-surface render (rgba_dev = nullptr: into the render's own image, read by render_image)
+int render_map_async(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_dev);
+const uint8_t* render_image(EfContext* ctx);
+void render_free(EfContext* ctx);
 }  // namespace ef

@@ -285,8 +285,48 @@ class GlobalModel {
     ef::check(ef_map_download(ctx_, out, (int32_t)n, &cnt), "downloadMap");
     return out;
   }
+  // GlobalModel::renderPointCloud (GlobalModel.cpp:286-350) with the reference's arguments, drawn into `rgba` (width * height * 4
+  // bytes, RGBA8, row 0 = window y 0, (0,0,0,0) where no surfel is drawn) instead of the bound framebuffer. mvp: column-major
+  // float[16], as the MVP uniform receives it. drawPoints (the draw_feedback point program) is outside this library's scope.
+  void renderPointCloud(const float* mvp, const float threshold, const bool drawUnstable, const bool drawNormals, const bool drawColors,
+                        const bool drawPoints, const bool drawWindow, const bool drawTimes, const int time, const int timeDelta, const int width,
+                        const int height, std::vector<uint8_t>& rgba) {
+    if (drawPoints) {
+      std::fprintf(stderr, "GlobalModel(b200): renderPointCloud with drawPoints (draw_feedback) is outside this library's scope.\n");
+      std::exit(1);
+    }
+    render(mvp, nullptr, threshold, drawUnstable, drawNormals, drawColors, drawWindow, drawTimes, time, timeDelta, false, false, width, height, rgba);
+  }
+  // The colour pass of GUI::drawFXAA (Tools/GUI.h:273-345): draw_global_surface_phong.frag, lit from the model-view's translation;
+  // invertNormals is the GUI's iclnuim flag (signMult = invertNormals ? 1 : -1). mv: column-major float[16].
+  void renderPhong(const float* mvp, const float* mv, const float threshold, const int time, const int timeDelta, const bool invertNormals,
+                   const bool drawUnstable, const bool drawNormals, const bool drawColors, const bool drawWindow, const bool drawTimes,
+                   const int width, const int height, std::vector<uint8_t>& rgba) {
+    render(mvp, mv, threshold, drawUnstable, drawNormals, drawColors, drawWindow, drawTimes, time, timeDelta, true, invertNormals, width, height, rgba);
+  }
 
  private:
+  void render(const float* mvp, const float* mv, float threshold, bool drawUnstable, bool drawNormals, bool drawColors, bool drawWindow,
+              bool drawTimes, int time, int timeDelta, bool phong, bool invertNormals, int width, int height, std::vector<uint8_t>& rgba) {
+    EfRenderView v = {};
+    v.width = width;
+    v.height = height;
+    for (int i = 0; i < 16; ++i) {
+      v.mvp[i] = mvp[i];
+      v.mv[i] = mv ? mv[i] : 0.f;
+    }
+    v.threshold = threshold;
+    v.color_type = drawNormals ? 1 : drawColors ? 2 : drawTimes ? 3 : 0;
+    v.unstable = drawUnstable;
+    v.draw_window = drawWindow;
+    v.time = time;
+    v.time_delta = timeDelta;
+    v.phong = phong;
+    v.sign_mult = invertNormals ? 1.f : -1.f;
+    rgba.resize((size_t)(width > 0 ? width : 0) * (height > 0 ? height : 0) * 4);
+    ef::check(ef_render_map(ctx_, &v, rgba.data()), phong ? "renderPhong" : "renderPointCloud");
+  }
+
   EfContext* ctx_;
   std::pair<uint32_t, uint32_t> handle_;
 };

@@ -277,6 +277,37 @@ int ef_map_upload_range(EfContext* ctx, const float* in12, int32_t first, int32_
 /* unstable surfels appended by the last ef_map_fuse (the reference's newUnstableVbo) */
 int ef_map_download_new(EfContext* ctx, float* out12, int32_t max_surfels, int32_t* count);
 
+/* ---- map render: the global-surface pass of the reference's viewer, GlobalModel::renderPointCloud (Core/GlobalModel.cpp:286-350,
+ *      drawPoints = false) and the colour pass of GUI::drawFXAA (Tools/GUI.h:273-345): every surfel drawn as a screen-facing disc by
+ *      draw_global_surface.{vert,geom,frag} / draw_global_surface_phong.frag, depth-tested GL_LESS against a 24-bit depth buffer.
+ *      The render has its own z-buffer and image (allocated by the first call, grown to the largest view, freed by ef_destroy) and
+ *      touches neither the frame's textures nor its pose state, so it may run between any two frames, also while a frame is staged by
+ *      the look-ahead or in flight between ef_process_frame_device and ef_finish_frame (it renders the map that frame leaves).
+ *
+ *      Output: RGBA8, W*H*4 bytes, in glReadPixels order: row 0 is window y = 0. Pixels no surfel covers are (0,0,0,0), so alpha is
+ *      coverage. colour_type 3 at time <= 1 divides by zero as the reference's geometry shader does; that output is not pinned. */
+typedef struct {
+  int32_t width, height;     /* 1..16384 */
+  float mvp[16];             /* column-major, the MVP uniform (pangolin::OpenGlMatrix cast to float, as Uniform does) */
+  float mv[16];              /* column-major model-view; read only when phong = 1 (lightpos = its translation) */
+  float threshold;           /* confidence threshold */
+  int32_t color_type;        /* 0 grey, 1 normals, 2 colours, 3 times: renderPointCloud's drawNormals/drawColors/drawTimes */
+  int32_t unstable, draw_window, time, time_delta;
+  int32_t phong;             /* 0: draw_global_surface.frag (renderPointCloud); 1: draw_global_surface_phong.frag (drawFXAA's colour pass) */
+  float sign_mult;           /* phong only; the GUI passes iclnuim ? 1 : -1 */
+} EfRenderView;
+/* EF_EINVAL for a size out of range, colour_type outside 0..3 or a non-finite matrix. Synchronises. */
+int ef_render_map(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_host);
+/* same into DEVICE memory (W*H*4 bytes), asynchronous on ef_stream() */
+int ef_render_map_device(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_dev);
+/* mvp16 / mv16 (column-major) of a pinhole camera at pose T_wc16 (row-major camera-to-world): mv = T_wc^-1, and a projection under
+ * which window pixel (i, j) samples the ray through image pixel centre (i + 0.5, j + 0.5) with rows as ef_map_raycast has them, so
+ * a render from the tracked pose with the frame's intrinsics lines up with the input image, top row first. Window depth 0 at
+ * z_near, 1 at z_far. EF_EINVAL for a size outside 1..16384, non-finite input, fx or fy = 0, or not 0 < z_near < z_far. No device
+ * work. */
+int ef_render_camera(const double* T_wc16, float fx, float fy, float cx, float cy, int32_t width, int32_t height, float z_near,
+                     float z_far, float* mvp16, float* mv16);
+
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
   /* input / preprocess textures (ElasticFusion::textures, GPUTexture.cpp:22-27) */

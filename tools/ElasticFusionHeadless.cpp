@@ -8,7 +8,10 @@
 //   -icl  -o  -rl(refused)  -fs  -q(implied)  -fo  -nso  -f  -ftf  -r(ignored: nothing to watch)
 // additions: -w <width> -h <height> (default 640 480), -cap <surfels>, -dev <cuda device>, -ply (write the map at the end),
 //            -nola (no frame look-ahead), -v (per-frame line), -dlc (without -o: close local loops inside processFrame, i.e.
-//            sample, solve and apply the deformation graph on the device; prints the number of closures applied)
+//            sample, solve and apply the deformation graph on the device; prints the number of closures applied),
+//            -render N (every N frames and after the last one, write <log>.render.<tick>.ppm: the map drawn as the reference's viewer
+//            draws it -- GlobalModel::renderPointCloud -- from the tracked pose at the input intrinsics and resolution, so it lines up
+//            with the input image), -rt T (its colour type: 0 grey, 1 normals, 2 colours (default), 3 times)
 #include <ElasticFusion.h>
 #include <Tools/RawLogReader.h>
 
@@ -23,6 +26,23 @@
 #include <string>
 
 namespace {
+
+// <log>.render.<tick>.ppm: the map from the current pose, as GlobalModel::renderPointCloud draws it (stable surfels only)
+void writeRender(ElasticFusion& eFusion, const std::string& logFile, int colorType, float confidence, int timeDelta) {
+  const int w = Resolution::getInstance().width(), h = Resolution::getInstance().height();
+  const Intrinsics& K = Intrinsics::getInstance();
+  double T[16];
+  ef::toRowMajor(eFusion.get_T_wc(), T);
+  float mvp[16], mv[16];
+  ef::check(ef_render_camera(T, K.fx(), K.fy(), K.cx(), K.cy(), w, h, 0.1f, 1000.0f, mvp, mv), "render camera");
+  std::vector<uint8_t> rgba;
+  eFusion.getGlobalModel().renderPointCloud(mvp, confidence, false, colorType == 1, colorType == 2, false, false, colorType == 3,
+                                            eFusion.getTick(), timeDelta, w, h, rgba);
+  const std::string path = logFile + ".render." + std::to_string(eFusion.getTick()) + ".ppm";
+  std::ofstream f(path, std::ios::binary);
+  f << "P6\n" << w << " " << h << "\n255\n";
+  for (size_t p = 0; p < (size_t)w * h; ++p) f.write(reinterpret_cast<const char*>(&rgba[p * 4]), 3);  // row 0 = the image's top row
+}
 
 int findArg(int argc, char** argv, const char* name) {
   for (int i = 1; i < argc; ++i)
@@ -112,7 +132,7 @@ int main(int argc, char** argv) {
   getArg(argc, argv, "-l", logFile);
   if (logFile.empty() || findArg(argc, argv, "--help") > 0) {
     std::fprintf(stderr, "usage: %s -l <log.klg> [-cal <file>] [-w W -h H] [-o] [-icl] [-fo] [-nso] [-f] [-ftf] [-c conf] [-d depth] [-i icp] "
-                         "[-t timeDelta] [-s start] [-e end] [-p poses] [-cap surfels] [-dev n] [-ply] [-nola] [-v] [-dlc]\n", argv[0]);
+                         "[-t timeDelta] [-s start] [-e end] [-p poses] [-cap surfels] [-dev n] [-ply] [-nola] [-v] [-dlc] [-render N] [-rt T]\n", argv[0]);
     return 2;
   }
   int width = 640, height = 480;
@@ -161,6 +181,15 @@ int main(int argc, char** argv) {
   const bool so3 = !(findArg(argc, argv, "-nso") > 0), frameToFrameRGB = findArg(argc, argv, "-ftf") > 0;
   const bool lookahead = !(findArg(argc, argv, "-nola") > 0) && !frameskip, verbose = findArg(argc, argv, "-v") > 0;
   const bool deviceLoopClosure = !openLoop && findArg(argc, argv, "-dlc") > 0;
+  int renderEvery = 0, renderType = 2;
+  getArg(argc, argv, "-render", renderEvery);
+  getArg(argc, argv, "-rt", renderType);
+  if (renderType < 0 || renderType > 3) {
+    std::fprintf(stderr, "-rt: colour type 0..3\n");
+    return 1;
+  }
+  const int renderTimeDelta = openLoop ? std::numeric_limits<int>::max() / 2 : timeDelta;
+  int lastRendered = -1;
 
   RawLogReader reader(logFile, flip);
   ElasticFusion eFusion(openLoop ? std::numeric_limits<int>::max() / 2 : timeDelta, icpCountThresh, icpErrThresh, covThresh, !openLoop, iclnuim, reloc,
@@ -197,7 +226,12 @@ int main(int argc, char** argv) {
       std::printf("frame %d tick %d t %.4f %.4f %.4f surfels %u %.3f ms\n", reader.currentFrame, eFusion.getTick(), (double)M(0, 3), (double)M(1, 3),
                   (double)M(2, 3), eFusion.getGlobalModel().lastCount(), ms);
     }
+    if (renderEvery > 0 && processed % renderEvery == 0) {
+      writeRender(eFusion, logFile, renderType, confidence, renderTimeDelta);
+      lastRendered = processed;
+    }
   }
+  if (renderEvery > 0 && processed > 0 && lastRendered != processed) writeRender(eFusion, logFile, renderType, confidence, renderTimeDelta);
   const double s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   std::printf("%d frames in %.3f s (%.1f frames/s incl. log decode), %u surfels, tick %d\n", processed, s, processed / (s > 0 ? s : 1),
               eFusion.getGlobalModel().lastCount(), eFusion.getTick());
