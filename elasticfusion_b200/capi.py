@@ -66,6 +66,27 @@ def camera_view(T_wc, fx, fy, cx, cy, w, h, near=0.1, far=1000.0, **flags) -> Ef
     return v
 
 
+class EfModelView(C.Structure):
+    _fields_ = [("T_wc", C.c_double * 16), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("width", C.c_int32),
+                ("height", C.c_int32), ("max_depth", C.c_float), ("conf_threshold", C.c_float), ("time", C.c_int32), ("max_time", C.c_int32),
+                ("time_delta", C.c_int32)]
+
+
+def model_view(T_wc, fx, fy, cx, cy, w, h, max_depth, conf_threshold, time, max_time, time_delta) -> EfModelView:
+    """EfModelView of combinedPredict at pose T_wc (4x4 camera-to-world) through a w x h pinhole camera. The time window is
+    combinedPredict's: ACTIVE = (tick, tick, time_delta), INACTIVE = (0, tick - time_delta, time_delta)."""
+    v = EfModelView()
+    v.T_wc[:] = [float(x) for x in np.asarray(T_wc, np.float64).reshape(16)]
+    v.fx, v.fy, v.cx, v.cy = float(fx), float(fy), float(cx), float(cy)
+    v.width, v.height = int(w), int(h)
+    v.max_depth, v.conf_threshold = float(max_depth), float(conf_threshold)
+    v.time, v.max_time, v.time_delta = int(time), int(max_time), int(time_delta)
+    return v
+
+
+# outputs of a model view: dtype and channels per pixel
+VIEW_OUTPUTS = {"image": (np.uint8, 4), "vertex": (np.float32, 4), "normal": (np.float32, 4), "time": (np.uint16, 1)}
+
 TRACE_DTYPE = np.dtype([
     ("kind", "<i4"), ("level", "<i4"), ("iter", "<i4"), ("rgb_count", "<i4"), ("rgb_sigma", "<i4"),
     ("sigma_val", "<f4"),
@@ -473,6 +494,22 @@ class Context:
     def render_device(self, view: EfRenderView, ptr):
         """ef_render_map_device: the same into device memory at ptr (H*W*4 bytes), asynchronous on the context's stream."""
         _chk(lib().ef_render_map_device(self.h_ctx, C.byref(view), C.c_void_p(ptr)))
+
+    def predict_view(self, view: EfModelView, outputs=("image", "vertex", "normal", "time")):
+        """ef_map_predict_view: combinedPredict at the view's pose, camera and size, without touching the frame. Returns a dict of the
+        requested outputs: image (H, W, 4) uint8, vertex and normal (H, W, 4) float32, time (H, W) uint16; row 0 is the top image
+        row, uncovered pixels are zero, the depth is vertex[..., 2]."""
+        out = {}
+        for name in outputs:
+            dt, ch = VIEW_OUTPUTS[name]
+            out[name] = np.zeros((view.height, view.width, ch) if ch > 1 else (view.height, view.width), dt)
+        _chk(lib().ef_map_predict_view(self.h_ctx, C.byref(view), *(_p(out.get(n)) for n in VIEW_OUTPUTS)))
+        return out
+
+    def predict_view_device(self, view: EfModelView, image=0, vertex=0, normal=0, time=0):
+        """ef_map_predict_view_device: the same into device memory (H*W*4, H*W*16, H*W*16, H*W*2 bytes; 0 = not wanted),
+        asynchronous on the context's stream."""
+        _chk(lib().ef_map_predict_view_device(self.h_ctx, C.byref(view), *(C.c_void_p(p or None) for p in (image, vertex, normal, time))))
 
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)

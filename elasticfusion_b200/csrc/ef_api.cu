@@ -197,6 +197,7 @@ static int create_buffers(EfContext* ctx) {
   CU(cudaEventCreateWithFlags(&la.h2d_done, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&la.image_ready, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&la.track_started, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&ctx->view_pose_sent, cudaEventDisableTiming));
   if (ctx->stage_timing) {
     CU(cudaEventCreate(&la.timing[0]));
     CU(cudaEventCreate(&la.timing[1]));
@@ -309,6 +310,7 @@ extern "C" int ef_destroy(EfContext* ctx) {
   if (ctx->la.h2d_done) cudaEventDestroy(ctx->la.h2d_done);
   if (ctx->la.image_ready) cudaEventDestroy(ctx->la.image_ready);
   if (ctx->la.track_started) cudaEventDestroy(ctx->la.track_started);
+  if (ctx->view_pose_sent) cudaEventDestroy(ctx->view_pose_sent);
   for (cudaEvent_t ev : ctx->la.timing)
     if (ev) cudaEventDestroy(ev);
   if (ctx->la.pin_rgb) cudaFreeHost(ctx->la.pin_rgb);
@@ -758,8 +760,11 @@ extern "C" int ef_render_map_device(EfContext* ctx, const EfRenderView* view, ui
 extern "C" int ef_render_map(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_host) {
   if (!ctx || !rgba_host || !render_view_ok(view)) return EF_EINVAL;
   CU(cudaSetDevice(ctx->device));
-  RC(render_map_async(ctx, view, nullptr));
-  CU(cudaMemcpyAsync(rgba_host, render_image(ctx), (size_t)view->width * view->height * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  const size_t bytes = (size_t)view->width * view->height * 4;
+  uint8_t* dev = nullptr;
+  RC(offframe_staging(ctx, bytes, &dev));
+  RC(render_map_async(ctx, view, dev));
+  CU(cudaMemcpyAsync(rgba_host, dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
@@ -790,6 +795,50 @@ extern "C" int ef_render_camera(const double* T_wc16, float fx, float fy, float 
       mvp16[c * 4 + r] = (float)acc;  // column-major
       mv16[c * 4 + r] = (float)mv[r * 4 + c];
     }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// model view: combinedPredict at any camera (ef_map.cu, on the render's z-buffer)
+// ---------------------------------------------------------------------------------------------------------------
+static bool model_view_ok(const EfModelView* v) {
+  if (!v || v->width < 1 || v->width > 16384 || v->height < 1 || v->height > 16384) return false;
+  for (int i = 0; i < 16; ++i)
+    if (!isfinite(v->T_wc[i])) return false;
+  return isfinite(v->fx) && isfinite(v->fy) && v->fx != 0.f && v->fy != 0.f && isfinite(v->cx) && isfinite(v->cy) && isfinite(v->max_depth) &&
+         v->max_depth > 0.f && isfinite(v->conf_threshold);
+}
+static bool aligned(const void* p, size_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
+extern "C" int ef_map_predict_view_device(EfContext* ctx, const EfModelView* v, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time) {
+  if (!ctx || !model_view_ok(v) || (!image4 && !vertex4 && !normal4 && !time)) return EF_EINVAL;
+  if (!aligned(image4, 4) || !aligned(vertex4, 16) || !aligned(normal4, 16) || !aligned(time, 2)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  return map_predict_view_async(ctx, v, image4, vertex4, normal4, time);
+}
+extern "C" int ef_map_predict_view(EfContext* ctx, const EfModelView* v, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time) {
+  if (!ctx || !model_view_ok(v) || (!image4 && !vertex4 && !normal4 && !time)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  // device staging of the requested outputs, the 16-byte ones first so that every part stays aligned
+  const size_t n = (size_t)v->width * v->height;
+  struct Part {
+    void* host;
+    size_t bytes;
+    uint8_t* dev;
+  } parts[4] = {{vertex4, n * 16, nullptr}, {normal4, n * 16, nullptr}, {image4, n * 4, nullptr}, {time, n * 2, nullptr}};
+  size_t total = 0;
+  for (Part& p : parts)
+    if (p.host) total += p.bytes;
+  uint8_t* dev = nullptr;
+  RC(offframe_staging(ctx, total, &dev));
+  for (Part& p : parts)
+    if (p.host) {
+      p.dev = dev;
+      dev += p.bytes;
+    }
+  RC(map_predict_view_async(ctx, v, parts[2].dev, (float*)parts[0].dev, (float*)parts[1].dev, (uint16_t*)parts[3].dev));
+  for (const Part& p : parts)
+    if (p.host) CU(cudaMemcpyAsync(p.host, p.dev, p.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
 

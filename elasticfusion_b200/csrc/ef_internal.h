@@ -161,6 +161,7 @@ struct MapDev {
   unsigned int* clean_ctl;   // [0] tile dispenser, [1] exit tickets, [2] first tile that moves (k_clean_flags -> k_clean_move)
   uint32_t* keep_mask;       // one warp ballot per 32 surfels: the clean test's verdicts
   MapPose* pose;         // device
+  MapPose* view_pose;    // device: the pose of ef_map_predict_view*, so that a view never touches the frame's `pose`
   int* dense_count;       // device: lit samples of the predicted image's decimation (dense_enough_of gives the flag)
   int* tick;              // device-resident tick
   float* nodes;           // deformation graph of the current frame, 16 floats per node
@@ -247,11 +248,13 @@ struct PinStaging {
   int finish_count;
   int loop_record[3];              // close_loops = 2, mid-frame: LoopDev::accepted, LoopDev::n_constraints, MapDev::graph_n
   EfDeformResult deform_result;    // close_loops = 2: the frame's deformation solve
+  double view_pose[16];  // map_predict_view_async: T_wc of a model view (rewritten after EfContext::view_pose_sent, not a sync)
 };
 // Layout of the device staging block (EfContext::dev_small): where the kernels read the pinned slots above.
 struct DevStaging {
   double map_pose[16];
   double T_wc[16];
+  double view_pose[16];
 };
 static_assert(sizeof(PinStaging) <= 65536 && sizeof(DevStaging) <= 65536, "staging blocks stay within 64 KiB");
 
@@ -305,7 +308,9 @@ struct EfContext {
   ef::DevStaging* dev_small;  // device side of the per-call parameters
   void* map_host;    // host-side bookkeeping of the surfel buffers (ef_map.cu)
   void* deform;      // workspace of the deformation-graph solve (ef_deform.cu), allocated by its first call
-  void* render;      // z-buffer and image of ef_render_map* (ef_render.cu), allocated by the first render and grown with the view
+  void* render;      // z-buffer and output staging of ef_render_map* and ef_map_predict_view* (ef_render.cu), allocated by the first
+                     // call and grown with the view
+  cudaEvent_t view_pose_sent;  // ctx->stream: the last model view's pose has been copied out of PinStaging::view_pose
   ef::Arena arena;   // every device buffer of the context
 };
 
@@ -431,6 +436,8 @@ int map_sample_graph_async(EfContext* ctx);
 // mode 0 also recounts dense_count; fill_in >= 0 (mode 0 only) also runs the fill-in in the same pass, with pass_img = fill_in
 int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode, int fill_in = -1);
 int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
+// combinedPredict at the view's pose, camera and size into the given device outputs (any may be null); touches no frame state
+int map_predict_view_async(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time);
 int map_dense_enough_async(EfContext* ctx);
 int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
 int map_loop_reset_async(EfContext* ctx);
@@ -448,8 +455,12 @@ int deform_solve_local(EfContext* ctx, const float4* graph, int n, const double*
                        bool pin, int src_time, int last_deform_time, EfDeformResult* out, const float** nodes16_dev);
 void deform_free(EfContext* ctx);
 
-// ef_render.cu: the global-surface render (rgba_dev = nullptr: into the render's own image, read by render_image)
+// ef_render.cu: the global-surface render, and the buffers of every pass outside the frame (the render and the model view), grown
+// to the largest view and freed by render_free
 int render_map_async(EfContext* ctx, const EfRenderView* view, uint8_t* rgba_dev);
-const uint8_t* render_image(EfContext* ctx);
+// n z-buffer keys, all kEmptyKey (~0) between passes: each pass's resolve re-arms the pixels its scatter may have written
+int offframe_zbuf(EfContext* ctx, size_t n, unsigned long long** out);
+// device staging of at least `bytes` (256-byte aligned) for a call that returns its outputs to the host
+int offframe_staging(EfContext* ctx, size_t bytes, uint8_t** out);
 void render_free(EfContext* ctx);
 }  // namespace ef

@@ -1334,6 +1334,8 @@ __device__ __forceinline__ bool is_dense_sample(int x, int size) {
 
 // Mode 0 (f.vertex != nullptr) also runs the fill-in of each pixel and counts the lit samples of denseEnough's decimation
 // into f.dense_count (zeroed by k_splat_scatter of the same raycast): the fill-in reads only pixel p of the outputs written here.
+// Without depth_out, each of image / vertex / normal / time_out is written only if given (the frame gives all four; a model
+// view may ask for any of them, and only when there is no fill-in).
 __global__ void k_splat_resolve(RayArgs a, const MapPose* __restrict__ mp, const float4* __restrict__ pos_conf,
                                 const float4* __restrict__ color_time, const float4* __restrict__ norm_rad,
                                 unsigned long long* __restrict__ zbuf, uchar4* __restrict__ image, float4* __restrict__ vertex,
@@ -1350,9 +1352,10 @@ __global__ void k_splat_resolve(RayArgs a, const MapPose* __restrict__ mp, const
       } else {
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
         const uchar4 z1 = make_uchar4(0, 0, 0, 0);
-        image[p] = z1;
-        vertex[p] = normal[p] = z4;
-        time_out[p] = 0;
+        if (image) image[p] = z1;
+        if (vertex) vertex[p] = z4;
+        if (normal) normal[p] = z4;
+        if (time_out) time_out[p] = 0;
         if (f.vertex) fill_in_pixel(f, a.rows, a.cols, a.c, px, py, p, z4, z4, z1);
       }
       continue;
@@ -1374,10 +1377,10 @@ __global__ void k_splat_resolve(RayArgs a, const MapPose* __restrict__ mp, const
     const float fxc = (float)px + 0.5f, fyc = (float)py + 0.5f;
     const float4 vt = make_float4((fxc - a.c.cx) * z * (1.f / a.c.fx), (fyc - a.c.cy) * z * (1.f / a.c.fy), z, sp.conf);
     const float4 nm = make_float4(sp.nrm.x, sp.nrm.y, sp.nrm.z, sp.rad);
-    image[p] = im;
-    vertex[p] = vt;
-    normal[p] = nm;
-    time_out[p] = (uint16_t)(unsigned int)ct.z;
+    if (image) image[p] = im;
+    if (vertex) vertex[p] = vt;
+    if (normal) normal[p] = nm;
+    if (time_out) time_out[p] = (uint16_t)(unsigned int)ct.z;
     if (f.dense_count && im.x > 0 && im.y > 0 && im.z > 0 && is_dense_sample(px, a.cols) && is_dense_sample(py, a.rows))
       atomicAdd(f.dense_count, 1);
     if (f.vertex) fill_in_pixel(f, a.rows, a.cols, a.c, px, py, p, vt, nm, im);
@@ -1533,6 +1536,7 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &B->fb_flag_raw, n));
   CU(ctx_alloc(ctx, &B->fb_flag_filt, n));
   CU(ctx_alloc(ctx, &m.pose, 1));
+  CU(ctx_alloc(ctx, &m.view_pose, 1));
   CU(ctx_alloc(ctx, &m.dense_count, 4, 0));
   CU(ctx_alloc(ctx, &m.tick, 4));
   CU(ctx_alloc(ctx, &m.nodes, (size_t)MAX_GRAPH_NODES * 16));
@@ -1774,6 +1778,36 @@ int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int
   }
   EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.zbuf, o.image, o.vertex, o.normal,
             o.time, o.depth, f);
+  CHECK_LAST();
+  return 0;
+}
+
+// the raycast above at the view's own pose, camera and size, on the off-frame z-buffer, with no fill-in and no dense count
+int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time) {
+  MapDev& m = ctx->map;
+  const size_t n = (size_t)v->width * v->height;
+  unsigned long long* zbuf = nullptr;
+  RC(offframe_zbuf(ctx, n, &zbuf));
+  // the staging slot is rewritten once the previous view's copy has read it (not the whole stream: the call stays asynchronous)
+  CU(cudaEventSynchronize(ctx->view_pose_sent));
+  memcpy(ctx->pin_small->view_pose, v->T_wc, sizeof(double) * 16);
+  CU(cudaMemcpyAsync(ctx->dev_small->view_pose, ctx->pin_small->view_pose, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaEventRecord(ctx->view_pose_sent, ctx->stream));
+  EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, m.view_pose, (const double*)ctx->dev_small->view_pose);
+  RayArgs a;
+  a.rows = v->height;
+  a.cols = v->width;
+  a.c = Cam{v->cx, v->cy, v->fx, v->fy};
+  a.max_depth = v->max_depth;
+  a.conf_threshold = v->conf_threshold;
+  a.time = v->time;
+  a.max_time = v->max_time;
+  a.time_delta = v->time_delta;
+  EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, m.count, zbuf,
+            (int*)nullptr);
+  EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, zbuf,
+            reinterpret_cast<uchar4*>(image), reinterpret_cast<float4*>(vertex), reinterpret_cast<float4*>(normal), time, (float*)nullptr,
+            FillOut{});
   CHECK_LAST();
   return 0;
 }

@@ -25,11 +25,12 @@ namespace {
 constexpr unsigned long long kEmptyKey = ~0ull;
 constexpr int RENDER_THREADS = 256;
 
-// the render's own buffers, grown to the largest view requested (ef_destroy frees them)
+// the buffers of the passes outside the frame (this render and the model view, ef_map.cu), grown to the largest view requested
+// (ef_destroy frees them)
 struct RenderBuffers {
-  unsigned long long* zbuf = nullptr;  // kept at kEmptyKey between renders by k_render_resolve
-  uchar4* image = nullptr;             // ef_render_map's device image
-  size_t zbuf_n = 0, image_n = 0;
+  unsigned long long* zbuf = nullptr;  // kept at kEmptyKey between passes by k_render_resolve / k_splat_resolve
+  uint8_t* staging = nullptr;          // device outputs of a call that returns them to the host
+  size_t zbuf_bytes = 0, staging_bytes = 0;
 };
 
 struct RenderQuad {
@@ -309,49 +310,59 @@ RenderBuffers* buffers(EfContext* ctx) {
   return static_cast<RenderBuffers*>(ctx->render);
 }
 
+// grows *p to at least `bytes` (never shrinks); true if it was reallocated
+template <typename T>
+int grow(EfContext* ctx, T** p, size_t& have, size_t bytes, bool* grown) {
+  *grown = bytes > have;
+  if (!*grown) return 0;
+  // (waits for the pass in flight that may still use the old buffer)
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (*p) CU(cudaFree(*p));
+  *p = nullptr;
+  have = 0;
+  CU(cudaMalloc((void**)p, bytes));
+  have = bytes;
+  return 0;
+}
+
 }  // namespace
 
 namespace ef {
 
-int render_map_async(EfContext* ctx, const EfRenderView* v, uint8_t* rgba_dev) {
+int offframe_zbuf(EfContext* ctx, size_t n, unsigned long long** out) {
   RenderBuffers* b = buffers(ctx);
-  const size_t n = (size_t)v->width * v->height;
-  if (n > b->zbuf_n) {
-    // (growing waits for the render in flight that may still use the old buffer)
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (b->zbuf) CU(cudaFree(b->zbuf));
-    b->zbuf = nullptr;
-    b->zbuf_n = 0;
-    CU(cudaMalloc(&b->zbuf, n * sizeof(unsigned long long)));
-    b->zbuf_n = n;
-    CU(cudaMemsetAsync(b->zbuf, 0xff, n * sizeof(unsigned long long), ctx->stream));
-  }
-  uchar4* out = reinterpret_cast<uchar4*>(rgba_dev);
-  if (!out) {
-    if (n > b->image_n) {
-      CU(cudaStreamSynchronize(ctx->stream));
-      if (b->image) CU(cudaFree(b->image));
-      b->image = nullptr;
-      b->image_n = 0;
-      CU(cudaMalloc(&b->image, n * sizeof(uchar4)));
-      b->image_n = n;
-    }
-    out = b->image;
-  }
-  const MapDev& m = ctx->map;
-  EF_LAUNCH(ctx, k_render_scatter, ctx->num_sms * 4, RENDER_THREADS, 0, *v, m.pos_conf, m.norm_rad, m.count, b->zbuf);
-  EF_LAUNCH(ctx, k_render_resolve, wave_blocks(ctx, n), 256, 0, *v, m.pos_conf, m.color_time, m.norm_rad, b->zbuf, out);
-  CHECK_LAST();
+  bool grown = false;
+  RC(grow(ctx, &b->zbuf, b->zbuf_bytes, n * sizeof(unsigned long long), &grown));
+  if (grown) CU(cudaMemsetAsync(b->zbuf, 0xff, b->zbuf_bytes, ctx->stream));
+  *out = b->zbuf;
   return 0;
 }
 
-const uint8_t* render_image(EfContext* ctx) { return ctx->render ? reinterpret_cast<const uint8_t*>(buffers(ctx)->image) : nullptr; }
+int offframe_staging(EfContext* ctx, size_t bytes, uint8_t** out) {
+  RenderBuffers* b = buffers(ctx);
+  bool grown = false;
+  RC(grow(ctx, &b->staging, b->staging_bytes, bytes, &grown));
+  *out = b->staging;
+  return 0;
+}
+
+int render_map_async(EfContext* ctx, const EfRenderView* v, uint8_t* rgba_dev) {
+  const size_t n = (size_t)v->width * v->height;
+  unsigned long long* zbuf = nullptr;
+  RC(offframe_zbuf(ctx, n, &zbuf));
+  uchar4* out = reinterpret_cast<uchar4*>(rgba_dev);
+  const MapDev& m = ctx->map;
+  EF_LAUNCH(ctx, k_render_scatter, ctx->num_sms * 4, RENDER_THREADS, 0, *v, m.pos_conf, m.norm_rad, m.count, zbuf);
+  EF_LAUNCH(ctx, k_render_resolve, wave_blocks(ctx, n), 256, 0, *v, m.pos_conf, m.color_time, m.norm_rad, zbuf, out);
+  CHECK_LAST();
+  return 0;
+}
 
 void render_free(EfContext* ctx) {
   RenderBuffers* b = static_cast<RenderBuffers*>(ctx->render);
   if (!b) return;
   if (b->zbuf) cudaFree(b->zbuf);
-  if (b->image) cudaFree(b->image);
+  if (b->staging) cudaFree(b->staging);
   delete b;
   ctx->render = nullptr;
 }

@@ -280,9 +280,10 @@ int ef_map_download_new(EfContext* ctx, float* out12, int32_t max_surfels, int32
 /* ---- map render: the global-surface pass of the reference's viewer, GlobalModel::renderPointCloud (Core/GlobalModel.cpp:286-350,
  *      drawPoints = false) and the colour pass of GUI::drawFXAA (Tools/GUI.h:273-345): every surfel drawn as a screen-facing disc by
  *      draw_global_surface.{vert,geom,frag} / draw_global_surface_phong.frag, depth-tested GL_LESS against a 24-bit depth buffer.
- *      The render has its own z-buffer and image (allocated by the first call, grown to the largest view, freed by ef_destroy) and
- *      touches neither the frame's textures nor its pose state, so it may run between any two frames, also while a frame is staged by
- *      the look-ahead or in flight between ef_process_frame_device and ef_finish_frame (it renders the map that frame leaves).
+ *      The render has its own z-buffer and output staging, shared with the model view below (allocated by the first call, grown to
+ *      the largest view, freed by ef_destroy), and touches neither the frame's textures nor its pose state, so it may run between
+ *      any two frames, also while a frame is staged by the look-ahead or in flight between ef_process_frame_device and
+ *      ef_finish_frame (it renders the map that frame leaves).
  *
  *      Output: RGBA8, W*H*4 bytes, in glReadPixels order: row 0 is window y = 0. Pixels no surfel covers are (0,0,0,0), so alpha is
  *      coverage. colour_type 3 at time <= 1 divides by zero as the reference's geometry shader does; that output is not pinned. */
@@ -307,6 +308,27 @@ int ef_render_map_device(EfContext* ctx, const EfRenderView* view, uint8_t* rgba
  * work. */
 int ef_render_camera(const double* T_wc16, float fx, float fy, float cx, float cy, int32_t width, int32_t height, float z_near,
                      float z_far, float* mvp16, float* mv16);
+
+/* ---- model view: IndexMap::combinedPredict (splat.vert + combo_splat.frag, Core/IndexMap.cpp:293-476) at any pose, intrinsics and
+ *      size. The outputs mean what EF_BUF_IMAGE / VERTEX / NORMAL / TIME mean after ef_map_raycast with the same arguments: row 0 is
+ *      the top image row, pixels no surfel covers are all zero, the depth is vertex.z. There is no fill-in (it needs the live frame,
+ *      which exists only at the frame's camera). A view touches no frame texture, pose record, z-buffer, index map or tracker state,
+ *      and uses the render's z-buffer (grown to the largest view, freed by ef_destroy), so like the render it may run between any two
+ *      frames, also while a frame is staged by the look-ahead or in flight between ef_process_frame_device and ef_finish_frame (it
+ *      predicts the map that frame leaves). */
+typedef struct {
+  double T_wc[16];                      /* row-major camera-to-world, as every pose in this ABI */
+  float fx, fy, cx, cy;
+  int32_t width, height;                /* 1..16384, as ef_render_map */
+  float max_depth, conf_threshold;
+  int32_t time, max_time, time_delta;   /* combinedPredict's window: ACTIVE = (tick, tick, td), INACTIVE = (0, tick - td, td) */
+} EfModelView;
+/* HOST outputs (W*H*4 B RGBA8, W*H*16 B float4 vertex + confidence, W*H*16 B float4 normal + radius, W*H*2 B time), synchronises.
+ * Any output may be NULL, but not all four. EF_EINVAL for all-NULL outputs, a size outside 1..16384, a non-finite pose entry, a
+ * non-finite or zero fx / fy, a non-finite cx / cy, max_depth not finite and > 0, or a non-finite conf_threshold. */
+int ef_map_predict_view(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time);
+/* same into DEVICE memory, asynchronous on ef_stream(); EF_EINVAL also for an output not aligned to its element (4, 16, 16, 2 B) */
+int ef_map_predict_view_device(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time);
 
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
