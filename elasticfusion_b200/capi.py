@@ -84,6 +84,25 @@ def model_view(T_wc, fx, fy, cx, cy, w, h, max_depth, conf_threshold, time, max_
     return v
 
 
+class EfFuseView(C.Structure):
+    _fields_ = [("T_wc", C.c_double * 16), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("width", C.c_int32),
+                ("height", C.c_int32), ("depth_cutoff", C.c_float), ("max_depth", C.c_float), ("weighting", C.c_float),
+                ("conf_threshold", C.c_float), ("time", C.c_int32), ("time_delta", C.c_int32)]
+
+
+def fuse_view(T_wc, fx, fy, cx, cy, w, h, time, weighting=1.0, depth_cutoff=3.0, max_depth=20.0, conf_threshold=10.0,
+              time_delta=200) -> EfFuseView:
+    """EfFuseView of an RGB-D frame taken at pose T_wc (4x4 camera-to-world) through a w x h pinhole camera, fused at tick `time`.
+    For the second camera of a rig, `time` is the tick of the tracked frame it accompanies (get_tick() - 1 after that frame)."""
+    v = EfFuseView()
+    v.T_wc[:] = [float(x) for x in np.asarray(T_wc, np.float64).reshape(16)]
+    v.fx, v.fy, v.cx, v.cy = float(fx), float(fy), float(cx), float(cy)
+    v.width, v.height = int(w), int(h)
+    v.depth_cutoff, v.max_depth, v.weighting, v.conf_threshold = float(depth_cutoff), float(max_depth), float(weighting), float(conf_threshold)
+    v.time, v.time_delta = int(time), int(time_delta)
+    return v
+
+
 # outputs of a model view: dtype and channels per pixel
 VIEW_OUTPUTS = {"image": (np.uint8, 4), "vertex": (np.float32, 4), "normal": (np.float32, 4), "time": (np.uint16, 1)}
 
@@ -510,6 +529,18 @@ class Context:
         """ef_map_predict_view_device: the same into device memory (H*W*4, H*W*16, H*W*16, H*W*2 bytes; 0 = not wanted),
         asynchronous on the context's stream."""
         _chk(lib().ef_map_predict_view_device(self.h_ctx, C.byref(view), *(C.c_void_p(p or None) for p in (image, vertex, normal, time))))
+
+    def fuse_view(self, view: EfFuseView, rgb, depth):
+        """ef_map_fuse_view: fuses an RGB-D frame of the view's camera into the map -- rgb (H, W, 3) uint8, depth (H, W) uint16
+        millimetres -- without touching the frame's pose, tick, textures or tracker state. Synchronises."""
+        r = np.ascontiguousarray(rgb, np.uint8)
+        d = np.ascontiguousarray(depth, np.uint16)
+        assert r.shape == (view.height, view.width, 3) and d.shape == (view.height, view.width), (r.shape, d.shape)
+        _chk(lib().ef_map_fuse_view(self.h_ctx, C.byref(view), _p(r), _p(d)))
+
+    def fuse_view_device(self, view: EfFuseView, rgb_ptr, depth_ptr):
+        """ef_map_fuse_view_device: the same from device memory (H*W*3 and H*W*2 bytes), asynchronous on the context's stream."""
+        _chk(lib().ef_map_fuse_view_device(self.h_ctx, C.byref(view), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None)))
 
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)

@@ -259,7 +259,6 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
     // level; 16 SMs are too few for the dense pass of the finer levels)
     e = getenv("EF_VISIBLE_LIST");
     ctx->visible_list = !(e && e[0] == '0');
-    ctx->vis_pending = false;
     e = getenv("EF_GN_CLUSTER");
     ctx->gn_cluster = odom_cluster_size(e ? atoi(e) : 16);
     e = getenv("EF_GN_CLUSTER_LEVELS");
@@ -318,6 +317,7 @@ extern "C" int ef_destroy(EfContext* ctx) {
   map_free_host(ctx);
   deform_free(ctx);
   render_free(ctx);
+  map_fuse_view_free(ctx);
   ctx->arena.release();
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
@@ -423,7 +423,7 @@ extern "C" int ef_upload(EfContext* ctx, int32_t id, int32_t level, const void* 
   if (bytes > b || !host) return EF_EINVAL;
   CU(cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
   if (id == EF_BUF_IMAGE) RC(map_dense_enough_async(ctx));  // the next frame's fill-in choice follows the uploaded image
-  if (id == EF_BUF_INDEX || id == EF_BUF_VERT_CONF || id == EF_BUF_COLOR_TIME || id == EF_BUF_NORM_RAD) ctx->index_keys_only = false;  // (only the frame path leaves them unwritten)
+  if (id == EF_BUF_INDEX || id == EF_BUF_VERT_CONF || id == EF_BUF_COLOR_TIME || id == EF_BUF_NORM_RAD) ctx->index.keys_only = false;  // (only the frame path leaves them unwritten)
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
@@ -615,7 +615,7 @@ extern "C" int ef_so3_step(EfContext* ctx, int which, const float* image_basis, 
 extern "C" int ef_preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,
                                    float* metric_filtered) {
   if (!ctx || !raw) return EF_EINVAL;
-  return preprocess_depth(ctx, raw, cutoff, filtered, metric, metric_filtered);
+  return preprocess_depth(ctx, ctx->cfg.height, ctx->cfg.width, raw, cutoff, filtered, metric, metric_filtered);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -672,24 +672,24 @@ extern "C" int ef_map_initialise(EfContext* ctx) {
 extern "C" int ef_map_predict_indices(EfContext* ctx, const double* T, int32_t time, float max_depth, int32_t time_delta) {
   if (!ctx) return EF_EINVAL;
   RC(map_update_pose_async(ctx, T));
-  return map_predict_indices_async(ctx, time, max_depth, time_delta);
+  return map_predict_indices_async(ctx, map_frame_target(ctx), time, max_depth, time_delta);
 }
 extern "C" int ef_map_fuse(EfContext* ctx, const double* T, int32_t time, float max_depth, float weighting) {
   if (!ctx) return EF_EINVAL;
   RC(map_update_pose_async(ctx, T));
-  return map_fuse_async(ctx, time, max_depth, weighting);
+  return map_fuse_async(ctx, map_frame_target(ctx), time, max_depth, weighting);
 }
 extern "C" int ef_map_clean(EfContext* ctx, const double* T, int32_t time, float conf_threshold, int32_t time_delta, float max_depth) {
   if (!ctx) return EF_EINVAL;
   RC(map_update_pose_async(ctx, T));
-  return map_clean_async(ctx, time, conf_threshold, time_delta, max_depth);
+  return map_clean_async(ctx, map_frame_target(ctx), time, conf_threshold, time_delta, max_depth);
 }
 extern "C" int ef_map_clean_deform(EfContext* ctx, const double* T, int32_t time, float conf_threshold, int32_t time_delta, float max_depth,
                                    const float* graph_nodes16, int32_t n_nodes, int32_t is_fern) {
   if (!ctx || n_nodes < 0 || (n_nodes > 0 && !graph_nodes16)) return EF_EINVAL;
   RC(map_set_graph(ctx, graph_nodes16, n_nodes));
   RC(map_update_pose_async(ctx, T));
-  return map_clean_async(ctx, time, conf_threshold, time_delta, max_depth, n_nodes, is_fern != 0);
+  return map_clean_async(ctx, map_frame_target(ctx), time, conf_threshold, time_delta, max_depth, n_nodes, is_fern != 0);
 }
 extern "C" int ef_map_raycast(EfContext* ctx, const double* T, float max_depth, float conf_threshold, int32_t time, int32_t max_time,
                               int32_t time_delta, int32_t mode) {
@@ -843,6 +843,57 @@ extern "C" int ef_map_predict_view(EfContext* ctx, const EfModelView* v, uint8_t
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// fuse view: the map half of a frame at any camera (ef_map.cu, on the view's own buffers)
+// ---------------------------------------------------------------------------------------------------------------
+static bool fuse_view_ok(const EfFuseView* v) {
+  if (!v || v->width < 1 || v->width > 16384 || v->height < 1 || v->height > 16384) return false;
+  for (int i = 0; i < 16; ++i)
+    if (!isfinite(v->T_wc[i])) return false;
+  return isfinite(v->fx) && isfinite(v->fy) && v->fx != 0.f && v->fy != 0.f && isfinite(v->cx) && isfinite(v->cy) &&
+         isfinite(v->depth_cutoff) && v->depth_cutoff > 0.f && isfinite(v->max_depth) && v->max_depth > 0.f && isfinite(v->weighting) &&
+         v->weighting >= 0.f && isfinite(v->conf_threshold) && v->time >= 0 && v->time_delta >= 0;
+}
+// before the first frame the map is not initialised (that frame would overwrite the view's surfels); between ef_process_frame_begin
+// and _end the frame's map half is still to come
+static int fuse_view_state(const EfContext* ctx) { return (ctx->tick <= 1 || ctx->frame_open) ? EF_ESTATE : 0; }
+
+// upload (host inputs), bilateral filter + metric depth, predictIndices, fuse, predictIndices, clean: ElasticFusion.cpp:536-584 with
+// no graph, at the view's camera
+static int fuse_view_async(EfContext* ctx, const EfFuseView* v, const uint8_t* rgb, const uint16_t* depth, bool from_host) {
+  MapTarget t;
+  uint8_t* rgb_buf = nullptr;
+  uint16_t* depth_buf = nullptr;
+  RC(map_fuse_view_target(ctx, v, &t, &rgb_buf, &depth_buf));
+  const size_t n = (size_t)v->width * v->height;
+  if (from_host) {
+    CU(cudaMemcpyAsync(rgb_buf, rgb, n * 3, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(depth_buf, depth, n * 2, cudaMemcpyHostToDevice, ctx->stream));
+    depth = depth_buf;
+  } else {
+    t.rgb = rgb;
+  }
+  RC(preprocess_depth(ctx, t.rows, t.cols, depth, v->depth_cutoff, nullptr, t.depth_metric, t.depth_metric_filtered));
+  RC(map_predict_indices_async(ctx, t, v->time, v->max_depth, v->time_delta));
+  RC(map_fuse_async(ctx, t, v->time, v->max_depth, -1.0f));  // (the view's weighting is staged with its pose)
+  RC(map_predict_indices_async(ctx, t, v->time, v->max_depth, v->time_delta));
+  return map_clean_async(ctx, t, v->time, v->conf_threshold, v->time_delta, v->max_depth);
+}
+
+extern "C" int ef_map_fuse_view_device(EfContext* ctx, const EfFuseView* v, const uint8_t* rgb_dev, const uint16_t* depth_dev) {
+  if (!ctx || !fuse_view_ok(v) || !rgb_dev || !depth_dev || !aligned(depth_dev, 2)) return EF_EINVAL;
+  RC(fuse_view_state(ctx));
+  CU(cudaSetDevice(ctx->device));
+  return fuse_view_async(ctx, v, rgb_dev, depth_dev, false);
+}
+extern "C" int ef_map_fuse_view(EfContext* ctx, const EfFuseView* v, const uint8_t* rgb, const uint16_t* depth) {
+  if (!ctx || !fuse_view_ok(v) || !rgb || !depth) return EF_EINVAL;
+  RC(fuse_view_state(ctx));
+  CU(cudaSetDevice(ctx->device));
+  RC(fuse_view_async(ctx, v, rgb, depth, true));
+  return ef_map_count(ctx, &ctx->host_count);  // (synchronises)
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // whole frame
 // ---------------------------------------------------------------------------------------------------------------
 // ElasticFusion::predict, reference Core/ElasticFusion.cpp:621-653 (lost == false, lastFrameRecovery == false)
@@ -867,7 +918,8 @@ static int frame_input_side(EfContext* ctx, const uint8_t* rgb_dev, const uint16
   if (depth_dev != t.depth_raw) CU(cudaMemcpyAsync(t.depth_raw, depth_dev, n * 2, cudaMemcpyDeviceToDevice, ctx->stream));
   RC(rgb_to_rgba(ctx, t.rgb, t.rgba));
   // filterDepth + metriciseDepth, ElasticFusion.cpp:284-285
-  RC(preprocess_depth(ctx, t.depth_raw, ctx->depth_cutoff, t.depth_filtered, t.depth_metric, t.depth_metric_filtered));
+  RC(preprocess_depth(ctx, ctx->cfg.height, ctx->cfg.width, t.depth_raw, ctx->depth_cutoff, t.depth_filtered, t.depth_metric,
+                      t.depth_metric_filtered));
   if (ctx->stream != ctx->la.stream) ef_stage(ctx, 1);  // (stage events live on the main stream only)
   // frameToModel.initICP(filtered depth) and the intensity half of initRGB, ElasticFusion.cpp:318-319
   RC(odom_init_icp_depth(ctx, 0, t.depth_filtered, ctx->max_depth_processed));
@@ -1043,15 +1095,16 @@ static int frame_begin_device(EfContext* ctx, const uint8_t* rgb_dev, const uint
 // Second half of processFrame (ElasticFusion.cpp:536-607): index map, fuse, index map, clean (with the deformation graph stored by
 // ef_set_deformation_graph when n_nodes > 0), predict, tick++.
 static int frame_map_device(EfContext* ctx, int n_nodes, bool fern_accepted) {
-  RC(map_predict_indices_async(ctx, ctx->tick, ctx->max_depth_processed, ctx->cfg.time_delta, 1));
+  const MapTarget t = map_frame_target(ctx);
+  RC(map_predict_indices_async(ctx, t, ctx->tick, ctx->max_depth_processed, ctx->cfg.time_delta, 1));
   ef_stage(ctx, 7);
-  RC(map_fuse_async(ctx, ctx->tick, ctx->max_depth_processed, -1.0f));
+  RC(map_fuse_async(ctx, t, ctx->tick, ctx->max_depth_processed, -1.0f));
   ef_stage(ctx, 8);
-  RC(map_predict_indices_async(ctx, ctx->tick, ctx->max_depth_processed, ctx->cfg.time_delta, 2));
+  RC(map_predict_indices_async(ctx, t, ctx->tick, ctx->max_depth_processed, ctx->cfg.time_delta, 2));
   ef_stage(ctx, 9);
   if (n_nodes > 0 && !fern_accepted)  // ElasticFusion.cpp:559-569: the time-stamp refresh of deformed surfels reads this depth
     RC(map_raycast_async(ctx, ctx->max_depth_processed, ctx->confidence, ctx->tick, ctx->tick - ctx->cfg.time_delta, 65535, 2));
-  RC(map_clean_async(ctx, ctx->tick, ctx->confidence, ctx->cfg.time_delta, ctx->max_depth_processed, n_nodes, fern_accepted));
+  RC(map_clean_async(ctx, t, ctx->tick, ctx->confidence, ctx->cfg.time_delta, ctx->max_depth_processed, n_nodes, fern_accepted));
   ef_stage(ctx, 10);
   return 0;
 }
@@ -1060,7 +1113,7 @@ static int frame_end_device(EfContext* ctx, int n_nodes, bool fern_accepted) {
   if (!ctx->frame_open) return EF_ESTATE;
   if (ctx->tick > 1 && !ctx->rgb_only) {
     if (int rc = frame_map_device(ctx, n_nodes, fern_accepted)) {
-      map_index_textures_async(ctx);  // a pass whose clean did not run still leaves its textures, as the stage API's passes do
+      map_index_textures_async(ctx, map_frame_target(ctx));  // a pass whose clean did not run still leaves its textures, as the stage API's passes do
       return rc;
     }
   }

@@ -149,19 +149,16 @@ struct MapDev {
   int* new_count;
   // per-pixel association scratch for fuse
   uint32_t* assoc_id;     // W*H: matched surfel id (or 0xffffffff none / 0xfffffffe new)
-  uint32_t* pending;      // capacity: lowest draw index that chose this surfel (0xffffffff idle)
+  uint32_t* pending;      // capacity: lowest draw index that chose this surfel (0xffffffff idle; every fuse leaves it so)
   // z-buffers
   unsigned long long* zbuf;        // W*H: the raycast's (k_splat_scatter / k_splat_resolve)
   unsigned long long* index_keys;  // W*H: the index map's tagged keys (IndexMap in ef_map.cu)
-  // scan scratch
-  int* scan_tile_state;   // decoupled look-back
-  unsigned int* scan_counter;
   uint32_t* vis_list;        // surfels that reached the z-buffer in the frame's first index-map pass (k_index_scatter<1>)
   int* vis_count;
   unsigned int* clean_ctl;   // [0] tile dispenser, [1] exit tickets, [2] first tile that moves (k_clean_flags -> k_clean_move)
   uint32_t* keep_mask;       // one warp ballot per 32 surfels: the clean test's verdicts
   MapPose* pose;         // device
-  MapPose* view_pose;    // device: the pose of ef_map_predict_view*, so that a view never touches the frame's `pose`
+  MapPose* view_pose;    // device: the pose of ef_map_predict_view* and ef_map_fuse_view*, so that a view never touches the frame's `pose`
   int* dense_count;       // device: lit samples of the predicted image's decimation (dense_enough_of gives the flag)
   int* tick;              // device-resident tick
   float* nodes;           // deformation graph of the current frame, 16 floats per node
@@ -248,15 +245,59 @@ struct PinStaging {
   int finish_count;
   int loop_record[3];              // close_loops = 2, mid-frame: LoopDev::accepted, LoopDev::n_constraints, MapDev::graph_n
   EfDeformResult deform_result;    // close_loops = 2: the frame's deformation solve
-  double view_pose[16];  // map_predict_view_async: T_wc of a model view (rewritten after EfContext::view_pose_sent, not a sync)
+  double view_pose[16];  // stage_view_pose: T_wc of a model or fuse view (rewritten after EfContext::view_pose_sent, not a sync)
+  float view_weighting;  // stage_view_pose: fusion weighting of a fuse view (same guard)
 };
 // Layout of the device staging block (EfContext::dev_small): where the kernels read the pinned slots above.
 struct DevStaging {
   double map_pose[16];
   double T_wc[16];
   double view_pose[16];
+  float view_weighting;
 };
 static_assert(sizeof(PinStaging) <= 65536 && sizeof(DevStaging) <= 65536, "staging blocks stay within 64 KiB");
+
+// Look-back tile states of order-preserving compactions (lookback_prefix) and their dispenser; each compaction takes a fresh epoch
+struct ScanTiles {
+  unsigned long long* state;
+  unsigned int* counter;
+  size_t bytes;
+  unsigned int epoch;
+};
+
+// Host-side state of one index map, kept across calls
+struct IndexState {
+  int pass;          // index-map passes since the keys were last re-armed: the current pass's tag is 0xff - pass
+  bool keys_only;    // the last index pass was a frame's: fuse and clean read its keys, the frame's clean writes its textures
+  bool vis_pending;  // the first pass of a frame has filled the visible list and no clean has re-armed it yet
+};
+
+// What the map's write side -- preprocess, index map, fuse, clean -- works on besides the surfels: a camera, its inputs, its index
+// map and the scratch sized by its pixels. The frame's (map_frame_target, rebuilt per call: the look-ahead swaps the input
+// buffers) or a fuse view's (map_fuse_view_target).
+struct MapTarget {
+  int rows, cols;
+  float cx, cy, fx, fy;
+  const uint8_t* rgb;  // W*H*3
+  float *depth_metric, *depth_metric_filtered;
+  const float* synth_depth;  // read by the clean's time-stamp refresh under a deformation graph (the frame's only)
+  MapPose* pose;
+  float* weighting;          // device: fuse's confidence weighting
+  // index map: tagged keys (key_texels of them, all re-armed when the tags run out) and the four textures
+  unsigned long long* index_keys;
+  size_t key_texels;
+  uint32_t* index;
+  float4 *vert_conf, *color_time, *norm_rad;
+  IndexState* ix;
+  // fuse: association per pixel and the unstable surfels it adds; clean: verdicts, control words and the kept count
+  uint32_t* assoc_id;
+  float4 *new_pos, *new_col, *new_nr;
+  int* new_count;
+  uint32_t* keep_mask;
+  unsigned int* clean_ctl;
+  int* clean_total;
+  ScanTiles* scan;  // covers the clean's capacity + W*H surfels and fuse's W*H pixels
+};
 
 }  // namespace ef
 
@@ -271,15 +312,13 @@ struct EfContext {
   cudaEvent_t stage_ev[16];
   int stage_n;
   bool pdl;  // programmatic dependent launch on every kernel (default on; EF_NO_PDL=1 disables)
-  bool vis_pending;      // the first pass of a frame has filled the visible list and no clean has re-armed it yet
   bool visible_list;      // second index-map pass of a frame visits only the surfels the first one rasterised; EF_VISIBLE_LIST=0 disables
   int gn_cluster;         // CTAs of the clusters that run the SO(3) loop and the coarse-level Gauss-Newton iterations (0: plain launches everywhere)
   int gn_cluster_levels;  // pyramid levels, from the coarsest, whose iterations run in that cluster
   bool la_after_track;    // the look-ahead's side stream starts after the frame's coarse-level cluster (EF_LA_AFTER_TRACK=0: at frame start)
   bool plain_next;     // the next ef_launch omits the programmatic-serialisation attribute (EF_PLAIN_NEXT)
   bool maps_dirty[2];  // a kernel that writes tracker w's pyramids may still be in flight ahead of the next stage launch
-  int index_pass;      // index-map passes since MapDev::index_keys was last re-armed: the current pass's tag is 0xff - index_pass
-  bool index_keys_only;  // the last index pass was a frame's: fuse and clean read its keys, the frame's clean writes its textures
+  ef::IndexState index;  // the frame's index map (MapDev::index_keys, Textures::index ...)
 
   ef::OdomDev odom[2];
   ef::MapDev map;
@@ -310,7 +349,9 @@ struct EfContext {
   void* deform;      // workspace of the deformation-graph solve (ef_deform.cu), allocated by its first call
   void* render;      // z-buffer and output staging of ef_render_map* and ef_map_predict_view* (ef_render.cu), allocated by the first
                      // call and grown with the view
-  cudaEvent_t view_pose_sent;  // ctx->stream: the last model view's pose has been copied out of PinStaging::view_pose
+  void* fuse_view;   // input, index-map and scratch buffers of ef_map_fuse_view* (ef_map.cu), allocated by the first call and grown
+                     // with the view
+  cudaEvent_t view_pose_sent;  // ctx->stream: the last view's pose and weighting have been copied out of PinStaging
   ef::Arena arena;   // every device buffer of the context
 };
 
@@ -409,8 +450,9 @@ int launch_rgb_residual_raw(EfContext* ctx, int which, int level);
 int launch_icp_dense_only(EfContext* ctx, int which, int level);
 int launch_so3_raw(EfContext* ctx, int which);
 
-// ef_preprocess.cu
-int preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric, float* metric_filtered);
+// ef_preprocess.cu: filtered / metric / metric_filtered may be null
+int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,
+                     float* metric_filtered);
 int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba);
 
 // ef_map.cu: the surfel map
@@ -425,11 +467,18 @@ struct ScanSlot {
 int scan_slot(EfContext* ctx, ScanSlot* out);
 int map_initialise_async(EfContext* ctx);
 int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
-int map_predict_indices_async(EfContext* ctx, int time_or_neg, float max_depth, int time_delta, int vis_mode = 0);
+// the frame's camera, inputs and buffers as they are now
+MapTarget map_frame_target(EfContext* ctx);
+// a fuse view's buffers, grown to the view (EF_ENOMEM if they cannot be: the context stays usable), with its pose and weighting
+// staged and uploaded to MapDev::view_pose; rgb / depth_raw: where its inputs may be uploaded (W*H*3, W*H)
+int map_fuse_view_target(EfContext* ctx, const EfFuseView* view, MapTarget* out, uint8_t** rgb, uint16_t** depth_raw);
+int map_predict_indices_async(EfContext* ctx, const MapTarget& t, int time, float max_depth, int time_delta, int vis_mode = 0);
 // the textures of a frame's index pass that no clean has written yet (nothing to do otherwise)
-int map_index_textures_async(EfContext* ctx);
-int map_fuse_async(EfContext* ctx, int time_or_neg, float max_depth, float weighting_or_neg);
-int map_clean_async(EfContext* ctx, int time_or_neg, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0, bool is_fern = false);
+int map_index_textures_async(EfContext* ctx, const MapTarget& t);
+// weighting < 0: the one *t.weighting already holds
+int map_fuse_async(EfContext* ctx, const MapTarget& t, int time, float max_depth, float weighting_or_neg);
+int map_clean_async(EfContext* ctx, const MapTarget& t, int time, float conf_threshold, int time_delta, float max_depth, int n_nodes = 0,
+                    bool is_fern = false);
 int map_set_graph(EfContext* ctx, const float* nodes16, int n_nodes);
 int map_set_graph_device(EfContext* ctx, const float* nodes16_dev, int n_nodes);
 int map_sample_graph_async(EfContext* ctx);
@@ -446,6 +495,7 @@ int map_download(EfContext* ctx, const float4* a, const float4* b, const float4*
 int map_upload(EfContext* ctx, const float* in, int n);
 int map_upload_range(EfContext* ctx, const float* in, int first, int n);
 int map_resize_to_host(EfContext* ctx, const void* src_dev, int elem, int factor, void* host_out);
+void map_fuse_view_free(EfContext* ctx);
 
 // ef_deform.cu: the deformation-graph solve
 int deform_solve(EfContext* ctx, const double* node_pos3, const int32_t* node_times, int n, const double* src3, const double* dst3,

@@ -13,6 +13,9 @@
 #include <float.h>
 #include <stddef.h>
 
+#include <new>
+#include <type_traits>
+
 #include "ef_device.cuh"
 #include "ef_dmath.cuh"
 #include "ef_internal.h"
@@ -647,7 +650,7 @@ __device__ __forceinline__ void fuse_update_item(const FuseArgs& a, const MapPos
 // of a tile take their slots in new_* from the tile's exclusive prefix (lookback_prefix), so they keep the draw order without a
 // separate scan; the last tile publishes the number of new surfels.
 constexpr int FU_THREADS = 128;
-__global__ void __launch_bounds__(FU_THREADS) k_fuse_update(FuseArgs a, const MapPose* __restrict__ mp, const GNState* __restrict__ gn,
+__global__ void __launch_bounds__(FU_THREADS) k_fuse_update(FuseArgs a, const MapPose* __restrict__ mp, const float* __restrict__ weighting_p,
                                                             const int* __restrict__ count, const uint32_t* __restrict__ assoc,
                                                             uint32_t* __restrict__ pending, float4* __restrict__ pos_conf,
                                                             float4* __restrict__ color_time, float4* __restrict__ norm_rad,
@@ -659,7 +662,7 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_update(FuseArgs a, const Ma
   const int nq = Q.ni * Q.nj;
   const int num_tiles = (nq + FU_THREADS - 1) / FU_THREADS;
   const int cnt = *count;
-  const float weighting = gn->weighting;
+  const float weighting = *weighting_p;
   __shared__ int s_warp[FU_THREADS / 32];
   __shared__ int s_tile, s_prefix;
   while (true) {
@@ -1445,6 +1448,7 @@ __global__ void k_unpack_aos(const float4* __restrict__ in, int n, float4* __res
 }
 
 inline Cam cam_of(const EfContext* ctx) { return Cam{ctx->cfg.cx, ctx->cfg.cy, ctx->cfg.fx, ctx->cfg.fy}; }
+inline Cam cam_of(const MapTarget& t) { return Cam{t.cx, t.cy, t.fx, t.fy}; }
 
 }  // namespace
 
@@ -1454,8 +1458,7 @@ struct MapBuffers {
   uint8_t *fb_flag_raw, *fb_flag_filt;
   float4* aos;  // staging for download/upload
   size_t aos_bytes;
-  unsigned int scan_epoch;  // tag of the current scan's tile states (k_scan_flags)
-  size_t scan_state_bytes;
+  ScanTiles scan;  // the frame's compactions (first-frame feedback, fuse, clean, the tracker's candidate list)
 };
 
 namespace ef {
@@ -1474,10 +1477,10 @@ static int aos_reserve(MapBuffers& B, size_t bytes) {
 }
 
 // next tag of the look-back tile states (every look-back compaction)
-static int next_scan_epoch(EfContext* ctx, MapBuffers& B) {
-  if (++B.scan_epoch >= (1u << 30)) {  // epoch field exhausted (never in practice): start over with clean states
-    CU(cudaMemsetAsync(ctx->map.scan_tile_state, 0, B.scan_state_bytes, ctx->stream));
-    B.scan_epoch = 1;
+static int next_scan_epoch(EfContext* ctx, ScanTiles& S) {
+  if (++S.epoch >= (1u << 30)) {  // epoch field exhausted (never in practice): start over with clean states
+    CU(cudaMemsetAsync(S.state, 0, S.bytes, ctx->stream));
+    S.epoch = 1;
   }
   return 0;
 }
@@ -1514,16 +1517,15 @@ int alloc_map(EfContext* ctx) {
   CU(ctx_alloc(ctx, &m.zbuf, n, 0xff));  // kept cleared by k_splat_resolve from here on
   // as if the tags had just run out: before the first pass re-arms it, no key carries the tag (0) fuse and clean look for
   CU(ctx_alloc(ctx, &m.index_keys, n, 0xff));
-  ctx->index_pass = 255;
-  ctx->index_keys_only = false;
+  ctx->index.pass = 255;
+  ctx->index.keys_only = false;
+  ctx->index.vis_pending = false;
   // look-back tile states: the clean pass walks capacity + n surfels in tiles of CC_TILE, the image-sized compactions
   // (first-frame feedback, new surfels, the tracker's candidate list) <= 2 n items in tiles of at least 128
   const size_t max_items = cap + n;
   const size_t tiles = (max_items + CC_TILE - 1) / CC_TILE + (2 * n + 127) / 128 + 2;
-  unsigned long long* st = nullptr;
-  CU(ctx_alloc(ctx, &st, tiles, 0));
-  m.scan_tile_state = reinterpret_cast<int*>(st);
-  CU(ctx_alloc(ctx, &m.scan_counter, 4, 0));
+  CU(ctx_alloc(ctx, &B->scan.state, tiles, 0));
+  CU(ctx_alloc(ctx, &B->scan.counter, 4, 0));
   CU(ctx_alloc(ctx, &m.clean_ctl, 4));
   CU(cudaMemsetAsync(m.clean_ctl, 0, 8, ctx->stream));
   CU(cudaMemsetAsync(m.clean_ctl + 2, 0xff, 8, ctx->stream));
@@ -1549,30 +1551,28 @@ int alloc_map(EfContext* ctx) {
     CU(ctx_alloc(ctx, &m.graph, (size_t)MAX_GRAPH_NODES - 1, 0));
     CU(ctx_alloc(ctx, &m.graph_n, 1, 0));
   }
-  B->scan_epoch = 0;
-  B->scan_state_bytes = tiles * 8;
+  B->scan.epoch = 0;
+  B->scan.bytes = tiles * 8;
   const int one = 1;
   CU(cudaMemcpyAsync(m.tick, &one, 4, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
 
-int scan_slot(EfContext* ctx, ScanSlot* out) {
-  MapBuffers& B = mb(ctx);
-  RC(next_scan_epoch(ctx, B));
-  out->state = (unsigned long long*)ctx->map.scan_tile_state;
-  out->counter = ctx->map.scan_counter;
-  out->epoch = B.scan_epoch;
+static int scan_slot_of(EfContext* ctx, ScanTiles& S, ScanSlot* out) {
+  RC(next_scan_epoch(ctx, S));
+  out->state = S.state;
+  out->counter = S.counter;
+  out->epoch = S.epoch;
   return 0;
 }
+int scan_slot(EfContext* ctx, ScanSlot* out) { return scan_slot_of(ctx, mb(ctx).scan, out); }
 
 static int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_b, size_t max_items, int* offsets, int* total) {
-  MapDev& m = ctx->map;
   const size_t tiles = (max_items + SCAN_TILE - 1) / SCAN_TILE + 1;
-  MapBuffers& B = mb(ctx);
-  RC(next_scan_epoch(ctx, B));
-  EF_LAUNCH(ctx, k_scan_flags, wave_blocks(ctx, tiles, 4, 1), SCAN_THREADS, 0, flags, n_a, n_b, offsets, (unsigned long long*)m.scan_tile_state, m.scan_counter, total,
-            B.scan_epoch);
+  ScanSlot sc;
+  RC(scan_slot(ctx, &sc));
+  EF_LAUNCH(ctx, k_scan_flags, wave_blocks(ctx, tiles, 4, 1), SCAN_THREADS, 0, flags, n_a, n_b, offsets, sc.state, sc.counter, total, sc.epoch);
   CHECK_LAST();
   return 0;
 }
@@ -1610,123 +1610,159 @@ int map_initialise_async(EfContext* ctx) {
   return 0;
 }
 
-static IndexMap index_map(EfContext* ctx) {
+MapTarget map_frame_target(EfContext* ctx) {
+  MapDev& m = ctx->map;
+  Textures& x = ctx->tex;
+  MapTarget t = {};
+  t.rows = m.rows;
+  t.cols = m.cols;
+  t.cx = ctx->cfg.cx;
+  t.cy = ctx->cfg.cy;
+  t.fx = ctx->cfg.fx;
+  t.fy = ctx->cfg.fy;
+  t.rgb = x.rgb;
+  t.depth_metric = x.depth_metric;
+  t.depth_metric_filtered = x.depth_metric_filtered;
+  t.synth_depth = x.synth_depth;
+  t.pose = m.pose;
+  t.weighting = &ctx->odom[0].gn->weighting;
+  t.index_keys = m.index_keys;
+  t.key_texels = (size_t)m.rows * m.cols;
+  t.index = x.index;
+  t.vert_conf = x.vert_conf;
+  t.color_time = x.color_time;
+  t.norm_rad = x.norm_rad;
+  t.ix = &ctx->index;
+  t.assoc_id = m.assoc_id;
+  t.new_pos = m.new_pos;
+  t.new_col = m.new_col;
+  t.new_nr = m.new_nr;
+  t.new_count = m.new_count;
+  t.keep_mask = m.keep_mask;
+  t.clean_ctl = m.clean_ctl;
+  t.clean_total = mb(ctx).totals + 3;
+  t.scan = &mb(ctx).scan;
+  return t;
+}
+
+static IndexMap index_map(const MapTarget& t) {
   IndexMap ix;
-  ix.keys = ctx->map.index_keys;
-  ix.tag = 0xffu - (unsigned int)ctx->index_pass;
-  ix.index = ctx->tex.index;
-  ix.vert_conf = ctx->tex.vert_conf;
-  ix.col_time = ctx->tex.color_time;
-  ix.norm_rad = ctx->tex.norm_rad;
+  ix.keys = t.index_keys;
+  ix.tag = 0xffu - (unsigned int)t.ix->pass;
+  ix.index = t.index;
+  ix.vert_conf = t.vert_conf;
+  ix.col_time = t.color_time;
+  ix.norm_rad = t.norm_rad;
   return ix;
 }
 
-// vis_mode 0: plain (stage API), textures written. 1: also record the surfels that reach the z-buffer (first pass of a frame).
-// 2: visit only those (second pass of the frame, same arguments, only fuse in between). The frame's passes (1, 2) leave the
-// textures to the frame's clean, which also re-arms the list.
-int map_predict_indices_async(EfContext* ctx, int time, float max_depth, int time_delta, int vis_mode) {
+// vis_mode 0: plain (stage API, fuse views), textures written. 1: also record the surfels that reach the z-buffer (first pass of
+// a frame). 2: visit only those (second pass of the frame, same arguments, only fuse in between). The frame's passes (1, 2) leave
+// the textures to the frame's clean, which also re-arms the list.
+int map_predict_indices_async(EfContext* ctx, const MapTarget& t, int time, float max_depth, int time_delta, int vis_mode) {
   MapDev& m = ctx->map;
-  const int n = m.rows * m.cols;
+  IndexState& st = *t.ix;
+  const int n = t.rows * t.cols;
   const bool in_frame = vis_mode != 0;
   if (!ctx->visible_list) vis_mode = 0;
   const int grid = ctx->num_sms * 5;
-  if (vis_mode == 1 && ctx->vis_pending) CU(cudaMemsetAsync(m.vis_count, 0, 4, ctx->stream));  // (a frame that failed before its clean)
-  if (vis_mode == 2 && !ctx->vis_pending) vis_mode = 0;
-  if (vis_mode == 1) ctx->vis_pending = true;
-  if (ctx->index_pass == 255) {  // the tags have run out: every key becomes stale
-    CU(cudaMemsetAsync(m.index_keys, 0xff, (size_t)n * sizeof(unsigned long long), ctx->stream));
-    ctx->index_pass = 0;
+  if (vis_mode == 1 && st.vis_pending) CU(cudaMemsetAsync(m.vis_count, 0, 4, ctx->stream));  // (a frame that failed before its clean)
+  if (vis_mode == 2 && !st.vis_pending) vis_mode = 0;
+  if (vis_mode == 1) st.vis_pending = true;
+  if (st.pass == 255) {  // the tags have run out: every key becomes stale
+    CU(cudaMemsetAsync(t.index_keys, 0xff, t.key_texels * sizeof(unsigned long long), ctx->stream));
+    st.pass = 0;
   }
-  ctx->index_pass++;
-  const IndexMap ix = index_map(ctx);
+  st.pass++;
+  const IndexMap ix = index_map(t);
   const auto scatter = vis_mode == 1 ? k_index_scatter<1> : vis_mode == 2 ? k_index_scatter<2> : k_index_scatter<0>;  // (mode 0 never reads the list)
-  EF_LAUNCH(ctx, scatter, grid, 256, 0, m.pos_conf, m.color_time, m.count, m.pose, time, max_depth, time_delta, m.rows, m.cols, cam_of(ctx),
-            m.index_keys, ix.tag, m.vis_list, m.vis_count, m.capacity);
-  ctx->index_keys_only = in_frame;
-  if (!in_frame) EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, ix, m.pos_conf, m.color_time, m.norm_rad, m.pose, n);
+  EF_LAUNCH(ctx, scatter, grid, 256, 0, m.pos_conf, m.color_time, m.count, t.pose, time, max_depth, time_delta, t.rows, t.cols, cam_of(t),
+            t.index_keys, ix.tag, m.vis_list, m.vis_count, m.capacity);
+  st.keys_only = in_frame;
+  if (!in_frame) EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, ix, m.pos_conf, m.color_time, m.norm_rad, t.pose, n);
   CHECK_LAST();
   return 0;
 }
 
-int map_index_textures_async(EfContext* ctx) {
-  if (!ctx->index_keys_only) return 0;
+int map_index_textures_async(EfContext* ctx, const MapTarget& t) {
+  if (!t.ix->keys_only) return 0;
   MapDev& m = ctx->map;
-  const int n = m.rows * m.cols;
-  EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, index_map(ctx), m.pos_conf, m.color_time, m.norm_rad, m.pose, n);
-  ctx->index_keys_only = false;
+  const int n = t.rows * t.cols;
+  EF_LAUNCH(ctx, k_index_textures, wave_blocks(ctx, n), 256, 0, index_map(t), m.pos_conf, m.color_time, m.norm_rad, t.pose, n);
+  t.ix->keys_only = false;
   CHECK_LAST();
   return 0;
 }
 
-static FuseArgs fuse_args(EfContext* ctx, int time, float max_depth) {
+static FuseArgs fuse_args(const MapTarget& t, int time, float max_depth) {
   FuseArgs a;
-  a.rgb = ctx->tex.rgb;
-  a.depth_raw = ctx->tex.depth_metric;
-  a.depth_filt = ctx->tex.depth_metric_filtered;
-  a.ix = index_map(ctx);
-  a.rows = ctx->map.rows;
-  a.cols = ctx->map.cols;
-  a.c = cam_of(ctx);
+  a.rgb = t.rgb;
+  a.depth_raw = t.depth_metric;
+  a.depth_filt = t.depth_metric_filtered;
+  a.ix = index_map(t);
+  a.rows = t.rows;
+  a.cols = t.cols;
+  a.c = cam_of(t);
   a.time = time;
   a.max_depth = max_depth;
   return a;
 }
 
-// weighting < 0: use the device-resident velocity weighting computed by the tracker
-int map_fuse_async(EfContext* ctx, int time, float max_depth, float weighting) {
+// weighting < 0: the device-resident one *t.weighting holds (the frame's: computed by the tracker)
+int map_fuse_async(EfContext* ctx, const MapTarget& t, int time, float max_depth, float weighting) {
   MapDev& m = ctx->map;
   if (weighting >= 0) {
     CU(cudaStreamSynchronize(ctx->stream));
     ctx->pin_small->weighting = weighting;
-    CU(cudaMemcpyAsync(&ctx->odom[0].gn->weighting, &ctx->pin_small->weighting, 4, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(t.weighting, &ctx->pin_small->weighting, 4, cudaMemcpyHostToDevice, ctx->stream));
   }
-  FuseArgs a = fuse_args(ctx, time, max_depth);
-  const Quarter Q = quarter_of(time, m.rows, m.cols);
+  FuseArgs a = fuse_args(t, time, max_depth);
+  const Quarter Q = quarter_of(time, t.rows, t.cols);
   const int nq = Q.ni * Q.nj;
-  const auto associate = ctx->index_keys_only ? k_fuse_associate<false> : k_fuse_associate<true>;
-  EF_LAUNCH(ctx, associate, wave_blocks(ctx, nq, 16, 128), 128, 0, a, m.pose, m.pos_conf, m.norm_rad, m.count, m.assoc_id, m.pending);
+  const auto associate = t.ix->keys_only ? k_fuse_associate<false> : k_fuse_associate<true>;
+  EF_LAUNCH(ctx, associate, wave_blocks(ctx, nq, 16, 128), 128, 0, a, t.pose, m.pos_conf, m.norm_rad, m.count, t.assoc_id, m.pending);
   ScanSlot sc;
-  RC(scan_slot(ctx, &sc));
-  EF_LAUNCH(ctx, k_fuse_update, wave_blocks(ctx, nq, 16, FU_THREADS), FU_THREADS, 0, a, m.pose, (const GNState*)ctx->odom[0].gn, m.count, m.assoc_id,
-            m.pending, m.pos_conf, m.color_time, m.norm_rad, m.new_pos, m.new_col, m.new_nr, m.new_count, sc.state, sc.counter, sc.epoch);
+  RC(scan_slot_of(ctx, *t.scan, &sc));
+  EF_LAUNCH(ctx, k_fuse_update, wave_blocks(ctx, nq, 16, FU_THREADS), FU_THREADS, 0, a, t.pose, (const float*)t.weighting, m.count, t.assoc_id,
+            m.pending, m.pos_conf, m.color_time, m.norm_rad, t.new_pos, t.new_col, t.new_nr, t.new_count, sc.state, sc.counter, sc.epoch);
   CHECK_LAST();
   return 0;
 }
 
 // n_nodes > 0: the deformation graph previously stored by map_set_graph is applied to every kept surfel
-int map_clean_async(EfContext* ctx, int time, float conf_threshold, int time_delta, float max_depth, int n_nodes, bool is_fern) {
+int map_clean_async(EfContext* ctx, const MapTarget& t, int time, float conf_threshold, int time_delta, float max_depth, int n_nodes,
+                    bool is_fern) {
   MapDev& m = ctx->map;
-  MapBuffers& B = mb(ctx);
+  IndexState& st = *t.ix;
   CleanArgs a;
-  a.ix = index_map(ctx);
-  a.rows = m.rows;
-  a.cols = m.cols;
-  a.c = cam_of(ctx);
+  a.ix = index_map(t);
+  a.rows = t.rows;
+  a.cols = t.cols;
+  a.c = cam_of(t);
   a.time = time;
   a.conf_threshold = conf_threshold;
   a.time_delta = time_delta;
   a.nodes = m.nodes;
   a.n_nodes = n_nodes;
-  a.depth = ctx->tex.synth_depth;
+  a.depth = t.synth_depth;
   a.max_depth = max_depth;
   a.is_fern = is_fern ? 1 : 0;
   // test (parallel) -> order-preserving in-place compaction + append of the new surfels + count publication (movers only)
-  const size_t max_items = (size_t)m.capacity + (size_t)m.rows * m.cols;
+  const size_t max_items = (size_t)m.capacity + (size_t)t.rows * t.cols;
   const size_t tiles = (max_items + CC_TILE - 1) / CC_TILE;
-  RC(next_scan_epoch(ctx, B));
+  RC(next_scan_epoch(ctx, *t.scan));
   // grids never depend on a surfel count the host would have to read back: the test strides over the tiles, the movers draw
   // tiles from a dispenser (one resident wave: four 49 KB CTAs per SM)
-  const int write_tex = ctx->index_keys_only ? 1 : 0;
-  int* reset_count = ctx->vis_pending ? m.vis_count : nullptr;
-  const auto flags = ctx->index_keys_only ? k_clean_flags<false> : k_clean_flags<true>;
-  EF_LAUNCH(ctx, flags, wave_blocks(ctx, tiles, 2, 1), CF_THREADS, 0, a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, m.new_pos,
-            m.new_col, m.new_nr, m.new_count, m.keep_mask, m.clean_ctl, write_tex, reset_count);
-  ctx->index_keys_only = false;
-  ctx->vis_pending = false;
+  const int write_tex = st.keys_only ? 1 : 0;
+  int* reset_count = st.vis_pending ? m.vis_count : nullptr;
+  const auto flags = st.keys_only ? k_clean_flags<false> : k_clean_flags<true>;
+  EF_LAUNCH(ctx, flags, wave_blocks(ctx, tiles, 2, 1), CF_THREADS, 0, a, t.pose, m.pos_conf, m.color_time, m.norm_rad, m.count, t.new_pos,
+            t.new_col, t.new_nr, t.new_count, t.keep_mask, t.clean_ctl, write_tex, reset_count);
+  st.keys_only = false;
+  st.vis_pending = false;
   const auto move = n_nodes > 0 ? k_clean_move<true> : k_clean_move<false>;
-  EF_LAUNCH(ctx, move, wave_blocks(ctx, tiles, 4, 1), CC_THREADS, sizeof(CcShared), a, m.pose, m.pos_conf, m.color_time, m.norm_rad, m.count,
-            m.new_pos, m.new_col, m.new_nr, m.new_count, m.capacity, m.keep_mask, (unsigned long long*)m.scan_tile_state, m.clean_ctl, B.totals + 3,
-            B.scan_epoch);
+  EF_LAUNCH(ctx, move, wave_blocks(ctx, tiles, 4, 1), CC_THREADS, sizeof(CcShared), a, t.pose, m.pos_conf, m.color_time, m.norm_rad, m.count,
+            t.new_pos, t.new_col, t.new_nr, t.new_count, m.capacity, t.keep_mask, t.scan->state, t.clean_ctl, t.clean_total, t.scan->epoch);
   CHECK_LAST();
   return 0;
 }
@@ -1782,18 +1818,31 @@ int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int
   return 0;
 }
 
+// a view's pose into MapDev::view_pose and, weighting >= 0, its fusion weighting into DevStaging::view_weighting. The pinned slots
+// are rewritten once the previous view's copies have read them (not the whole stream: the call stays asynchronous).
+static int stage_view_pose(EfContext* ctx, const double* T_wc, float weighting) {
+  PinStaging* pin = ctx->pin_small;
+  DevStaging* dev = ctx->dev_small;
+  CU(cudaEventSynchronize(ctx->view_pose_sent));
+  memcpy(pin->view_pose, T_wc, sizeof(double) * 16);
+  CU(cudaMemcpyAsync(dev->view_pose, pin->view_pose, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+  if (weighting >= 0) {
+    pin->view_weighting = weighting;
+    CU(cudaMemcpyAsync(&dev->view_weighting, &pin->view_weighting, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  }
+  CU(cudaEventRecord(ctx->view_pose_sent, ctx->stream));
+  EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, ctx->map.view_pose, (const double*)dev->view_pose);
+  CHECK_LAST();
+  return 0;
+}
+
 // the raycast above at the view's own pose, camera and size, on the off-frame z-buffer, with no fill-in and no dense count
 int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time) {
   MapDev& m = ctx->map;
   const size_t n = (size_t)v->width * v->height;
   unsigned long long* zbuf = nullptr;
   RC(offframe_zbuf(ctx, n, &zbuf));
-  // the staging slot is rewritten once the previous view's copy has read it (not the whole stream: the call stays asynchronous)
-  CU(cudaEventSynchronize(ctx->view_pose_sent));
-  memcpy(ctx->pin_small->view_pose, v->T_wc, sizeof(double) * 16);
-  CU(cudaMemcpyAsync(ctx->dev_small->view_pose, ctx->pin_small->view_pose, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
-  CU(cudaEventRecord(ctx->view_pose_sent, ctx->stream));
-  EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, m.view_pose, (const double*)ctx->dev_small->view_pose);
+  RC(stage_view_pose(ctx, v->T_wc, -1.0f));
   RayArgs a;
   a.rows = v->height;
   a.cols = v->width;
@@ -1810,6 +1859,134 @@ int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image,
             FillOut{});
   CHECK_LAST();
   return 0;
+}
+
+// ---- fuse view (ef_map_fuse_view*): its own inputs, index map and scratch, in one allocation grown to the largest view ----
+struct FuseViewBuffers {
+  void* block;
+  size_t px;  // pixels the block was carved for
+  uint8_t* rgb;
+  uint16_t* depth_raw;
+  float *depth_metric, *depth_metric_filtered;
+  unsigned long long* index_keys;
+  uint32_t* index;
+  float4 *vert_conf, *color_time, *norm_rad;
+  uint32_t* assoc_id;
+  float4 *new_pos, *new_col, *new_nr;
+  int *new_count, *clean_total;
+  unsigned int* clean_ctl;
+  uint32_t* keep_mask;
+  IndexState ix;
+  ScanTiles scan;
+};
+
+// carves the buffers of a px-pixel view out of `base` (nullptr: only sizes them); returns the bytes needed
+static size_t fuse_view_layout(FuseViewBuffers& V, uint8_t* base, size_t px, size_t capacity) {
+  size_t off = 0;
+  auto take = [&](auto** p, size_t bytes) {
+    off = (off + 255) & ~(size_t)255;
+    *p = base ? reinterpret_cast<std::remove_pointer_t<decltype(p)>>(base + off) : nullptr;
+    off += bytes;
+  };
+  const size_t clean_tiles = (capacity + px + CC_TILE - 1) / CC_TILE;
+  take(&V.rgb, px * 3);
+  take(&V.depth_raw, px * 2);
+  take(&V.depth_metric, px * 4);
+  take(&V.depth_metric_filtered, px * 4);
+  take(&V.index_keys, px * 8);
+  take(&V.index, px * 4);
+  take(&V.vert_conf, px * 16);
+  take(&V.color_time, px * 16);
+  take(&V.norm_rad, px * 16);
+  take(&V.assoc_id, px * 4);
+  take(&V.new_pos, px * 16);
+  take(&V.new_col, px * 16);
+  take(&V.new_nr, px * 16);
+  take(&V.new_count, 4);
+  take(&V.clean_total, 4);
+  take(&V.clean_ctl, 16);
+  take(&V.keep_mask, clean_tiles * CC_WORDS * 4);
+  take(&V.scan.counter, 8);
+  V.scan.bytes = (clean_tiles + (px + FU_THREADS - 1) / FU_THREADS + 2) * 8;  // the clean's tiles, or fuse's (at most px pixels)
+  take(&V.scan.state, V.scan.bytes);
+  return off;
+}
+
+int map_fuse_view_target(EfContext* ctx, const EfFuseView* v, MapTarget* out, uint8_t** rgb, uint16_t** depth_raw) {
+  if (!ctx->fuse_view) {
+    FuseViewBuffers* nv = new (std::nothrow) FuseViewBuffers();
+    if (!nv) return EF_ENOMEM;
+    ctx->fuse_view = nv;
+  }
+  FuseViewBuffers& V = *static_cast<FuseViewBuffers*>(ctx->fuse_view);
+  const size_t px = (size_t)v->width * v->height, cap = (size_t)ctx->map.capacity;
+  if (px > V.px) {
+    CU(cudaStreamSynchronize(ctx->stream));  // the previous view may still read the old block
+    if (V.block) CU(cudaFree(V.block));
+    V.block = nullptr;
+    V.px = 0;
+    const size_t bytes = fuse_view_layout(V, nullptr, px, cap);
+    if (cudaMalloc(&V.block, bytes) != cudaSuccess) {
+      V.block = nullptr;
+      cudaGetLastError();  // (an allocation failure is not sticky: the context stays usable)
+      return EF_ENOMEM;
+    }
+    fuse_view_layout(V, (uint8_t*)V.block, px, cap);
+    V.px = px;
+    // every key stale, no new surfels, clean's dispenser and tickets at zero and no first mover, no published tile state
+    CU(cudaMemsetAsync(V.index_keys, 0xff, px * sizeof(unsigned long long), ctx->stream));
+    CU(cudaMemsetAsync(V.new_count, 0, 4, ctx->stream));
+    CU(cudaMemsetAsync(V.clean_ctl, 0, 8, ctx->stream));
+    CU(cudaMemsetAsync(V.clean_ctl + 2, 0xff, 8, ctx->stream));
+    CU(cudaMemsetAsync(V.scan.counter, 0, 8, ctx->stream));
+    CU(cudaMemsetAsync(V.scan.state, 0, V.scan.bytes, ctx->stream));
+    V.scan.epoch = 0;
+    V.ix.pass = 0;
+    V.ix.keys_only = false;
+    V.ix.vis_pending = false;
+  }
+  RC(stage_view_pose(ctx, v->T_wc, v->weighting));
+  MapTarget t = {};
+  t.rows = v->height;
+  t.cols = v->width;
+  t.cx = v->cx;
+  t.cy = v->cy;
+  t.fx = v->fx;
+  t.fy = v->fy;
+  t.rgb = V.rgb;
+  t.depth_metric = V.depth_metric;
+  t.depth_metric_filtered = V.depth_metric_filtered;
+  t.synth_depth = nullptr;
+  t.pose = ctx->map.view_pose;
+  t.weighting = &ctx->dev_small->view_weighting;
+  t.index_keys = V.index_keys;
+  t.key_texels = V.px;
+  t.index = V.index;
+  t.vert_conf = V.vert_conf;
+  t.color_time = V.color_time;
+  t.norm_rad = V.norm_rad;
+  t.ix = &V.ix;
+  t.assoc_id = V.assoc_id;
+  t.new_pos = V.new_pos;
+  t.new_col = V.new_col;
+  t.new_nr = V.new_nr;
+  t.new_count = V.new_count;
+  t.keep_mask = V.keep_mask;
+  t.clean_ctl = V.clean_ctl;
+  t.clean_total = V.clean_total;
+  t.scan = &V.scan;
+  *out = t;
+  *rgb = V.rgb;
+  *depth_raw = V.depth_raw;
+  return 0;
+}
+
+void map_fuse_view_free(EfContext* ctx) {
+  FuseViewBuffers* V = static_cast<FuseViewBuffers*>(ctx->fuse_view);
+  if (!V) return;
+  if (V->block) cudaFree(V->block);
+  delete V;
+  ctx->fuse_view = nullptr;
 }
 
 int map_fill_in_async(EfContext* ctx, bool pass_geom, bool pass_img) {

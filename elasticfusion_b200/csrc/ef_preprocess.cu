@@ -68,8 +68,8 @@ __global__ void k_rgb_to_rgba(const uint8_t* __restrict__ rgb, uchar4* __restric
 }
 
 namespace ef {
-int preprocess_depth(EfContext* ctx, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric, float* metric_filtered) {
-  const int rows = ctx->cfg.height, cols = ctx->cfg.width;
+int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,
+                     float* metric_filtered) {
   dim3 grid((cols + TILE_X - 1) / TILE_X, (rows + TILE_Y - 1) / TILE_Y), block(TILE_X, TILE_Y);
   EF_LAUNCH(ctx, k_preprocess_depth, grid, block, 0, raw, rows, cols, cutoff, filtered, metric, metric_filtered);
   CHECK_LAST();

@@ -330,6 +330,42 @@ int ef_map_predict_view(EfContext* ctx, const EfModelView* view, uint8_t* image4
 /* same into DEVICE memory, asynchronous on ef_stream(); EF_EINVAL also for an output not aligned to its element (4, 16, 16, 2 B) */
 int ef_map_predict_view_device(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time);
 
+/* ---- fuse view: an RGB-D frame from any camera fused into the map, the map half of processFrame without a deformation graph
+ *      (Core/ElasticFusion.cpp:536-584) at a pose, intrinsics and size of the caller's choosing: upload, bilateral filter + metric
+ *      depth (depth_cutoff), predictIndices, fuse (weighting), predictIndices, clean (conf_threshold, time_delta), all at `time`
+ *      and max_depth. The map is byte-identical, order and count included, to what a context built for the view's camera (same
+ *      capacity) makes of the same map with ef_preprocess_depth, ef_map_predict_indices, ef_map_fuse, ef_map_predict_indices and
+ *      ef_map_clean with these arguments. A full map behaves as the frame's clean at capacity.
+ *
+ *      A view writes nothing but the surfels and their count: not the pose or tick, the frame's pose record or the tracker's
+ *      weighting, any EF_BUF_* texture, the denseEnough count, the unstable list of ef_map_download_new, the look-ahead's staged
+ *      frame or the loop-closure graph. Its inputs, index map and scratch are its own (allocated by the first call, grown to the
+ *      largest view, freed by ef_destroy). It does not refresh the predicted model: call ef_predict if the next frame should
+ *      track against the view's surfels.
+ *
+ *      For the second camera of a rig, `time` is the tick of the tracked frame the view accompanies (ef_get_tick() - 1 after it).
+ *      EF_ESTATE before the first frame (which initialises the map) and between ef_process_frame_begin and _end. Allowed while the
+ *      look-ahead holds a staged frame and between ef_process_frame_device and ef_finish_frame: the view is stream-ordered and
+ *      fuses into the map that frame leaves. */
+typedef struct {
+  double T_wc[16];           /* row-major camera-to-world */
+  float fx, fy, cx, cy;
+  int32_t width, height;     /* 1..16384 */
+  float depth_cutoff;        /* metric gate of the preprocess, metres (the frame uses cfg.depth_cutoff) */
+  float max_depth;           /* maxDepthProcessed (the frame uses 20) */
+  float weighting;           /* >= 0: fuse's confidence weighting, as ef_map_fuse takes it */
+  float conf_threshold;
+  int32_t time, time_delta;  /* the tick the view's surfels are stamped with; the index map's and clean's window */
+} EfFuseView;
+/* HOST inputs: RGB8 (W*H*3 B) and uint16 millimetres (W*H), as ef_process_frame takes them; synchronises. EF_EINVAL for a NULL
+ * input, a size outside 1..16384, a non-finite pose entry, a non-finite or zero fx / fy, a non-finite cx / cy, depth_cutoff or
+ * max_depth not finite and > 0, a negative or non-finite weighting, a non-finite conf_threshold, or time / time_delta < 0.
+ * EF_ENOMEM when the view's buffers cannot be grown (the context stays usable). */
+int ef_map_fuse_view(EfContext* ctx, const EfFuseView* view, const uint8_t* rgb, const uint16_t* depth);
+/* same from DEVICE inputs, asynchronous on ef_stream() (the inputs are read when the stream gets there); EF_EINVAL also for a depth
+ * pointer not aligned to 2 bytes */
+int ef_map_fuse_view_device(EfContext* ctx, const EfFuseView* view, const uint8_t* rgb_dev, const uint16_t* depth_dev);
+
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
   /* input / preprocess textures (ElasticFusion::textures, GPUTexture.cpp:22-27) */
