@@ -103,6 +103,41 @@ def fuse_view(T_wc, fx, fy, cx, cy, w, h, time, weighting=1.0, depth_cutoff=3.0,
     return v
 
 
+class EfOdomStats(C.Structure):
+    _fields_ = [("lastICPError", C.c_float), ("lastICPCount", C.c_float), ("lastRGBError", C.c_float), ("lastRGBCount", C.c_float),
+                ("lastSO3Error", C.c_float), ("lastSO3Count", C.c_float), ("lastA", C.c_double * 36), ("lastb", C.c_double * 6)]
+
+
+class EfTrackView(C.Structure):
+    _fields_ = [("model", EfModelView), ("depth_cutoff", C.c_float), ("icp_weight", C.c_float), ("rgb_only", C.c_int32),
+                ("pyramid", C.c_int32), ("fast_odom", C.c_int32)]
+
+
+class EfTrackResult(C.Structure):
+    _fields_ = [("T_wc", C.c_double * 16), ("stats", EfOdomStats), ("covariance", C.c_double * 36), ("dense_enough", C.c_int32)]
+
+
+def track_view(T_wc, fx, fy, cx, cy, w, h, time, max_time=None, time_delta=200, depth_cutoff=3.0, max_depth=20.0, conf_threshold=10.0,
+               icp_weight=10.0, rgb_only=False, pyramid=True, fast_odom=False) -> EfTrackView:
+    """EfTrackView of an RGB-D frame of a w x h pinhole camera, tracked against the map from the guess T_wc (4x4 camera-to-world).
+    The model is combinedPredict's window (time, max_time, time_delta); max_time None is `time`, the ACTIVE window the frame tracks
+    against at tick `time`. The defaults are the frame's: depth_cutoff 3 m, max_depth 20 m, confidence 10, icp_weight 10."""
+    v = EfTrackView()
+    v.model = model_view(T_wc, fx, fy, cx, cy, w, h, max_depth, conf_threshold, time, time if max_time is None else max_time, time_delta)
+    v.depth_cutoff, v.icp_weight = float(depth_cutoff), float(icp_weight)
+    v.rgb_only, v.pyramid, v.fast_odom = int(bool(rgb_only)), int(bool(pyramid)), int(bool(fast_odom))
+    return v
+
+
+def unpack_track_result(res):
+    """(T_wc (4, 4), stats (a STATS_DTYPE record, as Context.odom_stats), covariance (6, 6), dense_enough) of an EfTrackResult, or of
+    its bytes as ef_track_view_device wrote them."""
+    if not isinstance(res, EfTrackResult):
+        res = EfTrackResult.from_buffer_copy(bytes(res))
+    stats = np.frombuffer(bytes(res.stats), STATS_DTYPE)[0].copy()
+    return (np.array(res.T_wc[:]).reshape(4, 4), stats, np.array(res.covariance[:]).reshape(6, 6), bool(res.dense_enough))
+
+
 # outputs of a model view: dtype and channels per pixel
 VIEW_OUTPUTS = {"image": (np.uint8, 4), "vertex": (np.float32, 4), "normal": (np.float32, 4), "time": (np.uint16, 1)}
 
@@ -541,6 +576,27 @@ class Context:
     def fuse_view_device(self, view: EfFuseView, rgb_ptr, depth_ptr):
         """ef_map_fuse_view_device: the same from device memory (H*W*3 and H*W*2 bytes), asynchronous on the context's stream."""
         _chk(lib().ef_map_fuse_view_device(self.h_ctx, C.byref(view), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None)))
+
+    def track_view(self, view: EfTrackView, rgb, depth, max_trace=0):
+        """ef_track_view: tracks an RGB-D frame of the view's camera -- rgb (H, W, 3) uint8, depth (H, W) uint16 millimetres -- against
+        the map from the view's guess, without touching the frame. Synchronises. Returns (T_wc (4, 4), stats (as odom_stats),
+        covariance (6, 6), dense_enough, trace (the first max_trace Gauss-Newton records, TRACE_DTYPE))."""
+        h, w = view.model.height, view.model.width
+        r = np.ascontiguousarray(rgb, np.uint8)
+        d = np.ascontiguousarray(depth, np.uint16)
+        assert r.shape == (h, w, 3) and d.shape == (h, w), (r.shape, d.shape)
+        res = EfTrackResult()
+        trace = np.zeros(max(max_trace, 1), TRACE_DTYPE)
+        n = C.c_int32()
+        _chk(lib().ef_track_view(self.h_ctx, C.byref(view), _p(r), _p(d), C.byref(res), _p(trace) if max_trace else None, int(max_trace),
+                                 C.byref(n)))
+        return (*unpack_track_result(res), trace[:n.value].copy())
+
+    def track_view_device(self, view: EfTrackView, rgb_ptr, depth_ptr, result_ptr):
+        """ef_track_view_device: the same from device memory (H*W*3 and H*W*2 bytes) into an EfTrackResult in device memory
+        (ctypes.sizeof(EfTrackResult) bytes, 8-byte aligned; unpack_track_result reads its bytes), asynchronous on the context's stream."""
+        _chk(lib().ef_track_view_device(self.h_ctx, C.byref(view), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None),
+                                        C.c_void_p(result_ptr or None)))
 
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)

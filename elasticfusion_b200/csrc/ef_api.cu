@@ -53,11 +53,14 @@ extern "C" const char* ef_error_string(int code) {
   return "unknown error";
 }
 
-static int alloc_odom(EfContext* ctx, OdomDev& od) {
-  const EfConfig& c = ctx->cfg;
+namespace ef {
+int alloc_odom(EfContext* ctx, Arena& arena, int which, int width, int height, float fx, float fy, float cx, float cy) {
+  OdomDev& od = ctx->odom[which];
   memset(&od, 0, sizeof(od));
-  od.width = c.width;
-  od.height = c.height;
+  od.width = width;
+  od.height = height;
+  const float cam[4] = {fx, fy, cx, cy};
+  memcpy(ctx->odom_cam[which], cam, sizeof(cam));
   // RGBDOdometry ctor, reference Core/Utils/RGBDOdometry.cpp:22-117 and RGBDOdometry.h:41-42
   od.distThres = 0.10f;
   od.angleThres = sinf(20.f * 3.14159254f / 180.f);
@@ -69,41 +72,41 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
   od.minGrad[2] = 1;
   for (int i = 0; i < NUM_PYRS; ++i) {
     od.minScale[i] = (float)(pow((double)od.minGrad[i], 2.0) / pow((double)od.sobelScale, 2.0));
-    od.rows[i] = c.height >> i;
-    od.cols[i] = c.width >> i;
+    od.rows[i] = height >> i;
+    od.cols[i] = width >> i;
     const size_t n = (size_t)od.rows[i] * od.cols[i];
     // the reference's cudaMalloc'd maps start uninitialised; NaN / zero fill keeps every first read defined
-    CU(ctx_alloc(ctx, &od.depth_tmp[i], n, 0));
-    CU(ctx_alloc(ctx, &od.vmap_g_prev[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.nmap_g_prev[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.vmap_c_prev[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.nmap_c_prev[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.vmap_curr[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.nmap_curr[i], 3 * n, 0xff));
-    CU(ctx_alloc(ctx, &od.lastDepth[i], n, 0xff));
-    CU(ctx_alloc(ctx, &od.nextDepth[i], n, 0xff));
-    CU(ctx_alloc(ctx, &od.lastImage[i], n, 0));
-    CU(ctx_alloc(ctx, &od.nextImage[i], n, 0));
-    CU(ctx_alloc(ctx, &od.lastNextImage[i], n, 0));
-    CU(ctx_alloc(ctx, &od.dIdx[i], n, 0));
-    CU(ctx_alloc(ctx, &od.dIdy[i], n, 0));
-    CU(ctx_alloc(ctx, &od.corres[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.depth_tmp[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.vmap_g_prev[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.nmap_g_prev[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.vmap_c_prev[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.nmap_c_prev[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.vmap_curr[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.nmap_curr[i], 3 * n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.lastDepth[i], n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.nextDepth[i], n, 0xff));
+    CU(arena_alloc(ctx, arena, &od.lastImage[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.nextImage[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.lastNextImage[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.dIdx[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.dIdy[i], n, 0));
+    CU(arena_alloc(ctx, arena, &od.corres[i], n, 0));
   }
-  const size_t n0 = (size_t)c.width * c.height;
-  CU(ctx_alloc(ctx, &od.vmaps_tmp, 4 * n0, 0));
-  CU(ctx_alloc(ctx, &od.gn, 1));
+  const size_t n0 = (size_t)width * height;
+  CU(arena_alloc(ctx, arena, &od.vmaps_tmp, 4 * n0, 0));
+  CU(arena_alloc(ctx, arena, &od.gn, 1));
   od.cand_base = reinterpret_cast<const int*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, cand_base));
   od.intr0 = reinterpret_cast<const float*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, fx));
   od.K_levels = reinterpret_cast<const double*>(reinterpret_cast<const char*>(od.gn) + offsetof(GNState, Kd));
-  CU(ctx_alloc(ctx, &od.so3s, 1, 0));
+  CU(arena_alloc(ctx, arena, &od.so3s, 1, 0));
   // one slot per CTA of k_so3_step, whose grid red_blocks() caps at MAX_RED_BLOCKS (254 CTAs at 1920x1080 on an H100)
   // (the reductions read whole 32-float rows of the partials; the kernels write the 29 / 11 terms of a system, so the padding
   // lanes are defined once here)
-  CU(ctx_alloc(ctx, &od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
-  CU(ctx_alloc(ctx, &od.so3_counter, 4, 0));
-  CU(ctx_alloc(ctx, &od.partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
-  CU(ctx_alloc(ctx, &od.partials_rgb, (size_t)MAX_RGB_BLOCKS * 32, 0));
-  CU(ctx_alloc(ctx, &od.partials2, (size_t)MAX_RGB_BLOCKS * 32, 0));
+  CU(arena_alloc(ctx, arena, &od.so3_partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
+  CU(arena_alloc(ctx, arena, &od.so3_counter, 4, 0));
+  CU(arena_alloc(ctx, arena, &od.partials, (size_t)MAX_RED_BLOCKS * PARTIAL_STRIDE, 0));
+  CU(arena_alloc(ctx, arena, &od.partials_rgb, (size_t)MAX_RGB_BLOCKS * 32, 0));
+  CU(arena_alloc(ctx, arena, &od.partials2, (size_t)MAX_RGB_BLOCKS * 32, 0));
   {
     size_t flat = 0;
     for (int i = 0; i < NUM_PYRS; ++i) {
@@ -111,42 +114,25 @@ static int alloc_odom(EfContext* ctx, OdomDev& od) {
       flat += (size_t)od.rows[i] * od.cols[i];
     }
     od.level_start[NUM_PYRS] = (int)flat;
-    CU(ctx_alloc(ctx, &od.cand, flat, 0));
-    CU(ctx_alloc(ctx, &od.terms, flat, 0));
+    CU(arena_alloc(ctx, arena, &od.cand, flat, 0));
+    CU(arena_alloc(ctx, arena, &od.terms, flat, 0));
   }
-  CU(ctx_alloc(ctx, &od.partials_i, (size_t)MAX_RED_BLOCKS * 2));
-  CU(ctx_alloc(ctx, &od.counter, 4, 0));
-  CU(ctx_alloc(ctx, &od.trace, MAX_TRACE, 0));
+  CU(arena_alloc(ctx, arena, &od.partials_i, (size_t)MAX_RED_BLOCKS * 2));
+  CU(arena_alloc(ctx, arena, &od.counter, 4, 0));
+  CU(arena_alloc(ctx, arena, &od.trace, MAX_TRACE, 0));
   GNState g;
-  memset(&g, 0, sizeof(g));
-  for (int k = 0; k < 16; ++k) g.T_wc[k] = (k % 5 == 0) ? 1.0 : 0.0;
-  g.lastICPCount = g.lastRGBCount = g.lastSO3Count = (float)(c.width * c.height);
-  g.fx = c.fx;
-  g.fy = c.fy;
-  g.cx = c.cx;
-  g.cy = c.cy;
-  for (int lv = 0; lv < NUM_PYRS; ++lv) {
-    const int div = 1 << lv;  // CameraModel::operator()(level), reference Core/Cuda/types.cuh:92-95
-    const double fx = (double)(c.fx / div), fy = (double)(c.fy / div), cx = (double)(c.cx / div), cy = (double)(c.cy / div);
-    const double K[9] = {fx, 0, cx, 0, fy, cy, 0, 0, 1};
-    const double ifx = 1.0 / fx, ify = 1.0 / fy;
-    const double Ki[9] = {ifx, 0, -cx * ifx, 0, ify, -cy * ify, 0, 0, 1};
-    for (int k = 0; k < 9; ++k) {
-      g.Kd[lv][k] = K[k];
-      g.Kinvd[lv][k] = Ki[k];
-    }
-  }
-  g.break_level = -1;
-  g.weighting = 1.0f;
+  gn_initial_state(&g, width, height, fx, fy, cx, cy);
   CU(cudaMemcpyAsync(od.gn, &g, sizeof(g), cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
+  ctx->maps_dirty[which] = true;
   return 0;
 }
+}  // namespace ef
 
 // every buffer, stream and event of a context, in order; returns on the first error (ef_destroy frees whatever was made)
 static int create_buffers(EfContext* ctx) {
-  RC(alloc_odom(ctx, ctx->odom[0]));
-  RC(alloc_odom(ctx, ctx->odom[1]));
+  const EfConfig& c = ctx->cfg;
+  for (int w = 0; w < 2; ++w) RC(alloc_odom(ctx, ctx->arena, w, c.width, c.height, c.fx, c.fy, c.cx, c.cy));
   const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
   Textures& t = ctx->tex;
   memset(&t, 0, sizeof(t));
@@ -253,7 +239,7 @@ extern "C" int ef_create(const EfConfig* cfg, void* stream, EfContext** out) {
     const char* e = getenv("EF_NO_PDL");
     ctx->pdl = !(e && e[0] == '1');
     ctx->plain_next = false;
-    ctx->maps_dirty[0] = ctx->maps_dirty[1] = true;
+    for (bool& d : ctx->maps_dirty) d = true;
     // Gauss-Newton iterations of the coarse pyramid levels inside one thread-block cluster (k_gn_cluster): EF_GN_CLUSTER = wanted
     // cluster size (16 default, 8, or 0 = off), EF_GN_CLUSTER_LEVELS = how many levels from the top of the pyramid (default 1: the 160x120
     // level; 16 SMs are too few for the dense pass of the finer levels)
@@ -318,6 +304,7 @@ extern "C" int ef_destroy(EfContext* ctx) {
   deform_free(ctx);
   render_free(ctx);
   map_fuse_view_free(ctx);
+  track_view_free(ctx);
   ctx->arena.release();
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
@@ -894,6 +881,51 @@ extern "C" int ef_map_fuse_view(EfContext* ctx, const EfFuseView* v, const uint8
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// track view: the frame's tracking recipe at any camera (ef_track.cu, on the view's own buffers and tracker slot)
+// ---------------------------------------------------------------------------------------------------------------
+// the size rule of ef_create (every pyramid level at least 8 pixels on each side), capped at 4096 to bound the view's memory
+static bool track_view_ok(const EfTrackView* v) {
+  if (!v || !model_view_ok(&v->model)) return false;
+  const int w = v->model.width, h = v->model.height;
+  return w >= 32 && w <= 4096 && h >= 32 && h <= 4096 && (w >> 2) >= 8 && (h >> 2) >= 8 && isfinite(v->depth_cutoff) &&
+         v->depth_cutoff > 0.f && isfinite(v->icp_weight) && v->icp_weight >= 0.f;
+}
+
+extern "C" int ef_track_view_device(EfContext* ctx, const EfTrackView* v, const uint8_t* rgb_dev, const uint16_t* depth_dev, EfTrackResult* out_dev) {
+  if (!ctx || !track_view_ok(v) || !rgb_dev || !depth_dev || !out_dev || !aligned(depth_dev, 2) || !aligned(out_dev, 8)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  return track_view_async(ctx, v, rgb_dev, depth_dev, false, out_dev);
+}
+extern "C" int ef_track_view(EfContext* ctx, const EfTrackView* v, const uint8_t* rgb, const uint16_t* depth, EfTrackResult* out,
+                             EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace) {
+  if (!ctx || !track_view_ok(v) || !rgb || !depth || !out || max_trace < 0 || (max_trace > 0 && !trace)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  RC(track_view_async(ctx, v, rgb, depth, true, nullptr));
+  GNState g;
+  int lit = 0;
+  RC(track_view_read(ctx, &g, &lit));
+  memcpy(out->T_wc, g.T_wc, sizeof(g.T_wc));
+  EfOdomStats& s = out->stats;
+  s.lastICPError = g.lastICPError;
+  s.lastICPCount = g.lastICPCount;
+  s.lastRGBError = g.lastRGBError;
+  s.lastRGBCount = g.lastRGBCount;
+  s.lastSO3Error = g.lastSO3Error;
+  s.lastSO3Count = g.lastSO3Count;
+  memcpy(s.lastA, g.lastA, sizeof(g.lastA));
+  memcpy(s.lastb, g.lastb, sizeof(g.lastb));
+  efm::inv_n<6>(g.lastA, out->covariance);  // as ef_odom_covariance
+  out->dense_enough = dense_enough_of(lit, v->model.height, v->model.width) ? 1 : 0;
+  const int n = g.trace_n < max_trace ? g.trace_n : max_trace;
+  if (n_trace) *n_trace = n;
+  if (n > 0) {
+    CU(cudaMemcpyAsync(trace, ctx->odom[VIEW_TRACKER].trace, sizeof(EfSolveTrace) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // whole frame
 // ---------------------------------------------------------------------------------------------------------------
 // ElasticFusion::predict, reference Core/ElasticFusion.cpp:621-653 (lost == false, lastFrameRecovery == false)
@@ -916,7 +948,7 @@ static int frame_input_side(EfContext* ctx, const uint8_t* rgb_dev, const uint16
   // texture uploads, reference ElasticFusion.cpp:278-280
   if (rgb_dev != t.rgb) CU(cudaMemcpyAsync(t.rgb, rgb_dev, n * 3, cudaMemcpyDeviceToDevice, ctx->stream));
   if (depth_dev != t.depth_raw) CU(cudaMemcpyAsync(t.depth_raw, depth_dev, n * 2, cudaMemcpyDeviceToDevice, ctx->stream));
-  RC(rgb_to_rgba(ctx, t.rgb, t.rgba));
+  RC(rgb_to_rgba(ctx, ctx->cfg.height, ctx->cfg.width, t.rgb, t.rgba));
   // filterDepth + metriciseDepth, ElasticFusion.cpp:284-285
   RC(preprocess_depth(ctx, ctx->cfg.height, ctx->cfg.width, t.depth_raw, ctx->depth_cutoff, t.depth_filtered, t.depth_metric,
                       t.depth_metric_filtered));

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include <vector>
 
@@ -15,6 +16,10 @@ constexpr int RED_THREADS = 256;     // threads per reduction CTA
 constexpr int MAX_RED_BLOCKS = 1184; // 8 resident 256-thread CTAs per SM on up to 148 SMs (H100: 132)
 constexpr int PARTIAL_STRIDE = 64;   // floats per CTA partial: [0,29) geometric system, [32,61) photometric system
 constexpr int MAX_TRACE = 48;
+// tracker slots of EfContext::odom: 0 frameToModel, 1 modelToModel (both sized for the context's camera), and the tracker of
+// ef_track_view*, whose buffers are sized for the largest view so far
+constexpr int NUM_TRACKERS = 3;
+constexpr int VIEW_TRACKER = 2;
 constexpr int DENSE_FACTOR = 20;  // ElasticFusion::denseEnough decimates the predicted image by 20 (ElasticFusion.cpp:258)
 
 // ElasticFusion::denseEnough (ElasticFusion.cpp:256-268) from the number of lit samples of the decimated image
@@ -62,6 +67,32 @@ struct GNState {
   float weighting;  // velocity weighting for fusion (ElasticFusion.cpp:369-383)
   long long dbg[40];  // phase timestamps (%globaltimer) of levels 0 and 1 when built with -DEF_PROFILE_PHASES
 };
+
+// What a tracker's GNState holds before its first call (RGBDOdometry ctor, RGBDOdometry.cpp:22-117): identity pose, whole-image
+// counts, the level-0 intrinsics and K / K^-1 of every level. Written by alloc_odom on the host and, before every track view, on the
+// device, so that a view's result never depends on an earlier call.
+__host__ __device__ inline void gn_initial_state(GNState* g, int width, int height, float fx, float fy, float cx, float cy) {
+  memset(g, 0, sizeof(*g));
+  for (int k = 0; k < 16; ++k) g->T_wc[k] = (k % 5 == 0) ? 1.0 : 0.0;
+  g->lastICPCount = g->lastRGBCount = g->lastSO3Count = (float)(width * height);
+  g->fx = fx;
+  g->fy = fy;
+  g->cx = cx;
+  g->cy = cy;
+  for (int lv = 0; lv < NUM_PYRS; ++lv) {
+    const int div = 1 << lv;  // CameraModel::operator()(level), reference Core/Cuda/types.cuh:92-95
+    const double lfx = (double)(fx / div), lfy = (double)(fy / div), lcx = (double)(cx / div), lcy = (double)(cy / div);
+    const double K[9] = {lfx, 0, lcx, 0, lfy, lcy, 0, 0, 1};
+    const double ifx = 1.0 / lfx, ify = 1.0 / lfy;
+    const double Ki[9] = {ifx, 0, -lcx * ifx, 0, ify, -lcy * ify, 0, 0, 1};
+    for (int k = 0; k < 9; ++k) {
+      g->Kd[lv][k] = K[k];
+      g->Kinvd[lv][k] = Ki[k];
+    }
+  }
+  g->break_level = -1;
+  g->weighting = 1.0f;
+}
 
 // State of the SO(3) pre-alignment loop (RGBDOdometry.cpp:305-368). The loop depends only on the two intensity pyramids
 // (previous and current frame, level 2) -- not on the map, not on the pose -- so it has its own block, one per buffer set,
@@ -317,10 +348,11 @@ struct EfContext {
   int gn_cluster_levels;  // pyramid levels, from the coarsest, whose iterations run in that cluster
   bool la_after_track;    // the look-ahead's side stream starts after the frame's coarse-level cluster (EF_LA_AFTER_TRACK=0: at frame start)
   bool plain_next;     // the next ef_launch omits the programmatic-serialisation attribute (EF_PLAIN_NEXT)
-  bool maps_dirty[2];  // a kernel that writes tracker w's pyramids may still be in flight ahead of the next stage launch
+  bool maps_dirty[ef::NUM_TRACKERS];  // a kernel that writes tracker w's pyramids may still be in flight ahead of the next stage launch
   ef::IndexState index;  // the frame's index map (MapDev::index_keys, Textures::index ...)
 
-  ef::OdomDev odom[2];
+  ef::OdomDev odom[ef::NUM_TRACKERS];
+  float odom_cam[ef::NUM_TRACKERS][4];  // level-0 {fx, fy, cx, cy} of tracker w: the host's copy of what its GNState holds
   ef::MapDev map;
   ef::Textures tex;
   ef::Lookahead la;
@@ -351,6 +383,8 @@ struct EfContext {
                      // call and grown with the view
   void* fuse_view;   // input, index-map and scratch buffers of ef_map_fuse_view* (ef_map.cu), allocated by the first call and grown
                      // with the view
+  void* track_view;  // inputs, prediction and tracker buffers (odom[VIEW_TRACKER]) of ef_track_view* (ef_track.cu), allocated by the
+                     // first call and grown with the view
   cudaEvent_t view_pose_sent;  // ctx->stream: the last view's pose and weighting have been copied out of PinStaging
   ef::Arena arena;   // every device buffer of the context
 };
@@ -369,12 +403,17 @@ struct EfContext {
 #define CHECK_LAST() CU(cudaGetLastError())
 
 namespace ef {
-// n elements of T from the context's arena; fill >= 0: every byte set to `fill` on ctx->stream
+// n elements of T from `arena`; fill >= 0: every byte set to `fill` on ctx->stream
 template <typename T>
-inline cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n, int fill = -1) {
-  cudaError_t e = ctx->arena.alloc(p, n);
+inline cudaError_t arena_alloc(EfContext* ctx, Arena& arena, T** p, size_t n, int fill = -1) {
+  cudaError_t e = arena.alloc(p, n);
   if (e != cudaSuccess || fill < 0) return e;
   return cudaMemsetAsync(*p, fill, n * sizeof(T), ctx->stream);
+}
+// the same from the context's arena
+template <typename T>
+inline cudaError_t ctx_alloc(EfContext* ctx, T** p, size_t n, int fill = -1) {
+  return arena_alloc(ctx, ctx->arena, p, n, fill);
 }
 }  // namespace ef
 
@@ -430,6 +469,10 @@ inline int wave_blocks(const EfContext* ctx, size_t n, int per_sm = 8, int threa
 
 // ---- host entry points one translation unit calls in another; default arguments live here only -------------------
 namespace ef {
+// ef_api.cu: the buffers and initial state of tracker slot `which` (RGBDOdometry's constructor) for a width x height camera, from
+// `arena`; synchronises ctx->stream
+int alloc_odom(EfContext* ctx, Arena& arena, int which, int width, int height, float fx, float fy, float cx, float cy);
+
 // ef_track.cu: the tracker's input pyramids
 int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff);
 int odom_init_icp_pred(EfContext* ctx, int which, const float* vtx4, const float* nrm4);
@@ -438,6 +481,12 @@ int odom_populate(EfContext* ctx, int which, const uint8_t* rgba, float** destDe
                   bool with_image = true);
 int map_select_model_inputs(EfContext* ctx);
 int launch_sobel(EfContext* ctx, int which);
+// ef_track_view* (include/efusion_b200.h): host inputs when from_host (then out_dev may be null), device inputs otherwise; the
+// result packed into out_dev when given. The view tracker's state stays on the device for the host call to read.
+int track_view_async(EfContext* ctx, const EfTrackView* v, const uint8_t* rgb, const uint16_t* depth, bool from_host, EfTrackResult* out_dev);
+// the view tracker's GNState and the view's dense-sample count into host memory (synchronises)
+int track_view_read(EfContext* ctx, GNState* g, int* lit);
+void track_view_free(EfContext* ctx);
 
 // ef_reduce.cu: SO(3) loop, Gauss-Newton schedule and the stage API's reductions
 int odom_cluster_size(int want);
@@ -453,7 +502,7 @@ int launch_so3_raw(EfContext* ctx, int which);
 // ef_preprocess.cu: filtered / metric / metric_filtered may be null
 int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,
                      float* metric_filtered);
-int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba);
+int rgb_to_rgba(EfContext* ctx, int rows, int cols, const uint8_t* rgb, uint8_t* rgba);
 
 // ef_map.cu: the surfel map
 int alloc_map(EfContext* ctx);
@@ -465,6 +514,8 @@ struct ScanSlot {
   unsigned int epoch;
 };
 int scan_slot(EfContext* ctx, ScanSlot* out);
+// the same from a buffer set's own tile states
+int scan_slot(EfContext* ctx, ScanTiles& tiles, ScanSlot* out);
 int map_initialise_async(EfContext* ctx);
 int map_update_pose_async(EfContext* ctx, const double* T_host_or_null);
 // the frame's camera, inputs and buffers as they are now
@@ -485,8 +536,10 @@ int map_sample_graph_async(EfContext* ctx);
 // mode 0 also recounts dense_count; fill_in >= 0 (mode 0 only) also runs the fill-in in the same pass, with pass_img = fill_in
 int map_raycast_async(EfContext* ctx, float max_depth, float conf_threshold, int time, int max_time, int time_delta, int mode, int fill_in = -1);
 int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthrough_image);
-// combinedPredict at the view's pose, camera and size into the given device outputs (any may be null); touches no frame state
-int map_predict_view_async(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time);
+// combinedPredict at the view's pose, camera and size into the given device outputs (any may be null); touches no frame state.
+// dense_count: where the lit samples of the predicted image's decimation are counted (null: not counted)
+int map_predict_view_async(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time,
+                           int* dense_count = nullptr);
 int map_dense_enough_async(EfContext* ctx);
 int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
 int map_loop_reset_async(EfContext* ctx);

@@ -1567,6 +1567,7 @@ static int scan_slot_of(EfContext* ctx, ScanTiles& S, ScanSlot* out) {
   return 0;
 }
 int scan_slot(EfContext* ctx, ScanSlot* out) { return scan_slot_of(ctx, mb(ctx).scan, out); }
+int scan_slot(EfContext* ctx, ScanTiles& tiles, ScanSlot* out) { return scan_slot_of(ctx, tiles, out); }
 
 static int run_scan(EfContext* ctx, const uint8_t* flags, const int* n_a, const int* n_b, size_t max_items, int* offsets, int* total) {
   const size_t tiles = (max_items + SCAN_TILE - 1) / SCAN_TILE + 1;
@@ -1836,8 +1837,9 @@ static int stage_view_pose(EfContext* ctx, const double* T_wc, float weighting) 
   return 0;
 }
 
-// the raycast above at the view's own pose, camera and size, on the off-frame z-buffer, with no fill-in and no dense count
-int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time) {
+// the raycast above at the view's own pose, camera and size, on the off-frame z-buffer, with no fill-in; the dense count only
+// when asked for (a track view's)
+int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time, int* dense_count) {
   MapDev& m = ctx->map;
   const size_t n = (size_t)v->width * v->height;
   unsigned long long* zbuf = nullptr;
@@ -1853,10 +1855,11 @@ int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image,
   a.max_time = v->max_time;
   a.time_delta = v->time_delta;
   EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, m.count, zbuf,
-            (int*)nullptr);
+            dense_count);
+  FillOut f = {};
+  f.dense_count = dense_count;
   EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, zbuf,
-            reinterpret_cast<uchar4*>(image), reinterpret_cast<float4*>(vertex), reinterpret_cast<float4*>(normal), time, (float*)nullptr,
-            FillOut{});
+            reinterpret_cast<uchar4*>(image), reinterpret_cast<float4*>(vertex), reinterpret_cast<float4*>(normal), time, (float*)nullptr, f);
   CHECK_LAST();
   return 0;
 }

@@ -75,8 +75,8 @@ int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, fl
   CHECK_LAST();
   return 0;
 }
-int rgb_to_rgba(EfContext* ctx, const uint8_t* rgb, uint8_t* rgba) {
-  const size_t n = (size_t)ctx->cfg.height * ctx->cfg.width;
+int rgb_to_rgba(EfContext* ctx, int rows, int cols, const uint8_t* rgb, uint8_t* rgba) {
+  const size_t n = (size_t)rows * cols;
   EF_LAUNCH(ctx, k_rgb_to_rgba, wave_blocks(ctx, n), 256, 0, rgb, (uchar4*)rgba, n);
   CHECK_LAST();
   return 0;

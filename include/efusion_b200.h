@@ -366,6 +366,56 @@ int ef_map_fuse_view(EfContext* ctx, const EfFuseView* view, const uint8_t* rgb,
  * pointer not aligned to 2 bytes */
 int ef_map_fuse_view_device(EfContext* ctx, const EfFuseView* view, const uint8_t* rgb_dev, const uint16_t* depth_dev);
 
+/* ---- track view: an RGB-D frame from any camera tracked against the map, the frame-to-model recipe of processFrame
+ *      (Core/ElasticFusion.cpp:309-323) run by an RGBDOdometry of the view's camera (RGBDOdometry.cpp:22-117), from a pose guess of
+ *      the caller's: upload, RGBA, bilateral filter (depth_cutoff), the live depth pyramid and vertex / normal maps (initICP at
+ *      model.max_depth) and intensity pyramid, combinedPredict of `model` at the guess (no fill-in), initICPModel + initRGBModel
+ *      from it, Sobel and the photometric candidates, and getIncrementalTransformation(guess, rgb_only, icp_weight, pyramid,
+ *      fast_odom, so3 = false). As in the frame, initRGB's depth pyramid is the model's (quirk A.2). The result is byte-identical to
+ *      what a context built for the view's camera gives with ef_map_predict_view_device, ef_odom_init_icp_model(0, vertex, normal,
+ *      guess), ef_odom_init_rgb_model(0, image), ef_preprocess_depth, ef_odom_init_icp_depth(0, filtered, max_depth),
+ *      ef_odom_init_rgb(0, rgba) and ef_odom_track(0, guess, ..., so3 = 0), then ef_odom_stats and ef_odom_covariance.
+ *
+ *      There is no SO(3) pre-alignment and no fill-in: both need the previous live frame of the same camera, and a one-off view has
+ *      none (the reference's own trackers that are not the frame's, modelToModel and the fern tracker, also run with so3 = false).
+ *      dense_enough says how well the map covers the view, as ElasticFusion::denseEnough would decide for its predicted image.
+ *
+ *      A view only reads the map. It writes none of: the pose, tick or weighting of the frame, any EF_BUF_* buffer (the pyramids of
+ *      trackers 0 and 1 included), ef_odom_stats(0 / 1), the SO(3) state or staged frame of the look-ahead, the loop-closure state,
+ *      the denseEnough count, ef_debug_stage_ms's events or the map. Its inputs, prediction and tracker buffers are its own
+ *      (allocated by the first call, grown to the bounding box of the views so far, freed by ef_destroy): 243 B per pixel of that
+ *      box, plus 8 B per pixel for the z-buffer it shares with the render and the model view, and about 1 MB besides: 78 MB at
+ *      640x480, 521 MB at 1920x1080 and 4.2 GB at 4096x4096. It returns no EF_ESTATE: it may run before the first
+ *      frame (on a map from ef_map_upload), between ef_process_frame_begin and _end, while the look-ahead holds a staged frame and
+ *      between ef_process_frame_device and ef_finish_frame (stream-ordered: it tracks against the map that frame leaves).
+ *
+ *      On an empty map, or where the view sees no surfel, the call still returns 0 with whatever the recipe gives: no term is valid,
+ *      every system is zero, the pose is the guess as the tracker's finish rebuilds it from its float rotation, both counts are 0,
+ *      lastICPError is 0/0 (NaN), the covariance (the inverse of the zero lastA) is not finite and dense_enough is 0. */
+typedef struct {
+  EfModelView model;         /* the prediction tracked against, as ef_map_predict_view takes it. model.T_wc is the initial guess;
+                                model.max_depth is also initICP's cutoff (the frame uses 20 for both). width, height: 32..4096 */
+  float depth_cutoff;        /* > 0: the bilateral filter's maxD, metres (the frame uses cfg.depth_cutoff) */
+  float icp_weight;          /* >= 0 (the frame uses 10; >= 100: ICP only) */
+  int32_t rgb_only, pyramid, fast_odom;  /* as ef_odom_track takes them (the frame uses 0, 1, cfg.fast_odom) */
+} EfTrackView;
+typedef struct {
+  double T_wc[16];           /* tracked pose, row-major camera-to-world */
+  EfOdomStats stats;         /* as ef_odom_stats reports them */
+  double covariance[36];     /* lastA^-1, as ef_odom_covariance (RGBDOdometry::getCovariance) */
+  int32_t dense_enough;      /* ElasticFusion::denseEnough of the view's predicted image, at the view's size */
+} EfTrackResult;
+/* HOST inputs: RGB8 (W*H*3 B) and uint16 millimetres (W*H); synchronises. trace (HOST, may be NULL when max_trace = 0) receives one
+ * record per Gauss-Newton iteration, as ef_odom_track's. EF_EINVAL for a NULL input or output, a negative max_trace, each bad
+ * `model` field as ef_map_predict_view checks it, a size outside 32..4096, a non-finite or non-positive depth_cutoff, or a
+ * non-finite or negative icp_weight. EF_ENOMEM when the view's buffers cannot be grown (the context stays usable). */
+int ef_track_view(EfContext* ctx, const EfTrackView* view, const uint8_t* rgb, const uint16_t* depth, EfTrackResult* out,
+                  EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace);
+/* same from DEVICE inputs into a DEVICE result, asynchronous on ef_stream() (the inputs are read when the stream gets there); the
+ * covariance is computed on the device. EF_EINVAL also for a depth pointer not aligned to 2 bytes or out_dev not aligned to 8 */
+int ef_track_view_device(EfContext* ctx, const EfTrackView* view, const uint8_t* rgb_dev, const uint16_t* depth_dev,
+                         EfTrackResult* out_dev);
+
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
   /* input / preprocess textures (ElasticFusion::textures, GPUTexture.cpp:22-27) */
