@@ -138,6 +138,59 @@ def unpack_track_result(res):
     return (np.array(res.T_wc[:]).reshape(4, 4), stats, np.array(res.covariance[:]).reshape(6, 6), bool(res.dense_enough))
 
 
+class EfCameraConfig(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
+                ("depth_cutoff", C.c_float), ("max_depth", C.c_float), ("conf_threshold", C.c_float), ("time_delta", C.c_int32),
+                ("icp_weight", C.c_float), ("rgb_only", C.c_int32), ("pyramid", C.c_int32), ("fast_odom", C.c_int32), ("so3", C.c_int32),
+                ("frame_to_frame_rgb", C.c_int32)]
+
+
+class EfCameraFrame(C.Structure):
+    _fields_ = [("time", C.c_int32), ("weight_multiplier", C.c_float), ("has_pose", C.c_int32), ("T_wc", C.c_double * 16),
+                ("fuse", C.c_int32)]
+
+
+class EfCameraResult(C.Structure):
+    _fields_ = [("T_wc", C.c_double * 16), ("stats", EfOdomStats), ("covariance", C.c_double * 36), ("tracked", C.c_int32),
+                ("dense_enough", C.c_int32), ("weighting", C.c_float)]
+
+
+MAX_CAMERAS = 4  # EF_MAX_CAMERAS
+
+
+def camera_config(w, h, fx, fy, cx, cy, depth_cutoff=3.0, max_depth=20.0, conf_threshold=10.0, time_delta=200, icp_weight=10.0,
+                  rgb_only=False, pyramid=True, fast_odom=False, so3=True, frame_to_frame_rgb=False) -> EfCameraConfig:
+    """EfCameraConfig of a w x h pinhole camera. The defaults are the frame's (ef_default_config and the ElasticFusion constructor):
+    depth_cutoff 3 m, maxDepthProcessed 20 m, confidence 10, time_delta 200, icp_weight 10, pyramid and SO(3) on."""
+    c = EfCameraConfig()
+    c.width, c.height = int(w), int(h)
+    c.fx, c.fy, c.cx, c.cy = float(fx), float(fy), float(cx), float(cy)
+    c.depth_cutoff, c.max_depth, c.conf_threshold = float(depth_cutoff), float(max_depth), float(conf_threshold)
+    c.time_delta, c.icp_weight = int(time_delta), float(icp_weight)
+    c.rgb_only, c.pyramid, c.fast_odom = int(bool(rgb_only)), int(bool(pyramid)), int(bool(fast_odom))
+    c.so3, c.frame_to_frame_rgb = int(bool(so3)), int(bool(frame_to_frame_rgb))
+    return c
+
+
+def camera_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfCameraFrame:
+    """EfCameraFrame: the frame is stamped and predicted at `time`; T_wc (4x4 camera-to-world) sets the pose instead of tracking."""
+    f = EfCameraFrame()
+    f.time, f.weight_multiplier, f.fuse = int(time), float(weight_multiplier), int(bool(fuse))
+    if T_wc is not None:
+        f.has_pose = 1
+        f.T_wc[:] = np.asarray(T_wc, np.float64).reshape(16).tolist()
+    return f
+
+
+def unpack_camera_result(res):
+    """(T_wc (4, 4), stats (STATS_DTYPE), covariance (6, 6), {tracked, dense_enough, weighting}) of an EfCameraResult or its bytes."""
+    if not isinstance(res, EfCameraResult):
+        res = EfCameraResult.from_buffer_copy(bytes(res))
+    stats = np.frombuffer(bytes(res.stats), STATS_DTYPE)[0].copy()
+    info = dict(tracked=bool(res.tracked), dense_enough=bool(res.dense_enough), weighting=float(res.weighting))
+    return np.array(res.T_wc[:]).reshape(4, 4), stats, np.array(res.covariance[:]).reshape(6, 6), info
+
+
 # outputs of a model view: dtype and channels per pixel
 VIEW_OUTPUTS = {"image": (np.uint8, 4), "vertex": (np.float32, 4), "normal": (np.float32, 4), "time": (np.uint16, 1)}
 
@@ -598,6 +651,67 @@ class Context:
         _chk(lib().ef_track_view_device(self.h_ctx, C.byref(view), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None),
                                         C.c_void_p(result_ptr or None)))
 
+    def camera(self, cfg: EfCameraConfig) -> "Camera":
+        """ef_camera_create: a camera of this context (at most MAX_CAMERAS live ones)."""
+        return Camera(self, cfg)
+
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)
         _chk(lib().ef_map_upload(self.h_ctx, _p(s), len(s)))
+
+
+class Camera:
+    """One EfCamera of a Context: a second RGB-D sensor run frame after frame against the context's map (include/efusion_b200.h)."""
+
+    def __init__(self, ctx: Context, cfg: EfCameraConfig):
+        self.ctx, self.cfg = ctx, cfg
+        self.w, self.h = cfg.width, cfg.height
+        self.h_cam = C.c_void_p()
+        _chk(lib().ef_camera_create(ctx.h_ctx, C.byref(cfg), C.byref(self.h_cam)))
+
+    def close(self):
+        """ef_camera_destroy (a no-op once the camera or its context is closed)"""
+        if getattr(self, "h_cam", None) and self.ctx.h_ctx:
+            _chk(lib().ef_camera_destroy(self.ctx.h_ctx, self.h_cam))
+        self.h_cam = None
+
+    def frame(self, rgb, depth, time, weight_multiplier=1.0, T_wc=None, fuse=True, max_trace=0):
+        """ef_camera_frame: rgb (H, W, 3) uint8, depth (H, W) uint16 millimetres; T_wc sets the pose instead of tracking. Synchronises.
+        Returns (T_wc (4, 4), stats (as Context.odom_stats), covariance (6, 6), {tracked, dense_enough, weighting}, trace (the first
+        max_trace Gauss-Newton records of a tracked frame, TRACE_DTYPE))."""
+        r = np.ascontiguousarray(rgb, np.uint8)
+        d = np.ascontiguousarray(depth, np.uint16)
+        assert r.shape == (self.h, self.w, 3) and d.shape == (self.h, self.w), (r.shape, d.shape)
+        f = camera_frame(time, weight_multiplier, T_wc, fuse)
+        res = EfCameraResult()
+        trace = np.zeros(max(max_trace, 1), TRACE_DTYPE)
+        n = C.c_int32()
+        _chk(lib().ef_camera_frame(self.ctx.h_ctx, self.h_cam, C.byref(f), _p(r), _p(d), C.byref(res), _p(trace) if max_trace else None,
+                                   int(max_trace), C.byref(n)))
+        return (*unpack_camera_result(res), trace[:n.value].copy())
+
+    def frame_device(self, rgb_ptr, depth_ptr, result_ptr, time, weight_multiplier=1.0, T_wc=None, fuse=True):
+        """ef_camera_frame_device: the same from device memory (H*W*3 and H*W*2 bytes) into an EfCameraResult in device memory
+        (ctypes.sizeof(EfCameraResult) bytes, 8-byte aligned; unpack_camera_result reads its bytes), asynchronous on the context's stream."""
+        f = camera_frame(time, weight_multiplier, T_wc, fuse)
+        _chk(lib().ef_camera_frame_device(self.ctx.h_ctx, self.h_cam, C.byref(f), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None),
+                                          C.c_void_p(result_ptr or None)))
+
+    def buffer_ptr(self, name, level=0):
+        ptr, nbytes = C.c_void_p(), C.c_size_t()
+        _chk(lib().ef_camera_buffer(self.ctx.h_ctx, self.h_cam, BUF[name], level, C.byref(ptr), C.byref(nbytes)))
+        return ptr.value, nbytes.value
+
+    def download(self, name, level=0):
+        """A buffer of the camera (ef_camera_buffer: its inputs, prediction, fill-in and pyramids) as Context.download shapes it."""
+        bid = BUF[name]
+        dt, kind = _BUF_FMT[bid]
+        r, c = (self.h >> level, self.w >> level) if bid >= 40 and bid != 53 else (self.h, self.w)
+        shape = (r, c) if kind == "c1" else (3 * r, c) if kind == "p3" else (r, c, int(kind[1]))
+        out = np.zeros(shape, dt)
+        ptr, nbytes = self.buffer_ptr(name, level)
+        assert nbytes == out.nbytes, (name, nbytes, out.nbytes)
+        self.ctx.sync()
+        # cudaMemcpy of the CUDA runtime the library links (device to host = 2)
+        _chk(lib().cudaMemcpy(_p(out), C.c_void_p(ptr), C.c_size_t(nbytes), 2))
+        return out

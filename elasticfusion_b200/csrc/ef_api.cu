@@ -305,6 +305,8 @@ extern "C" int ef_destroy(EfContext* ctx) {
   render_free(ctx);
   map_fuse_view_free(ctx);
   track_view_free(ctx);
+  for (EfCamera* cam : ctx->cameras)
+    if (cam) camera_destroy(ctx, cam);
   ctx->arena.release();
   if (ctx->pin_rgb) cudaFreeHost(ctx->pin_rgb);
   if (ctx->pin_depth) cudaFreeHost(ctx->pin_depth);
@@ -331,6 +333,30 @@ extern "C" int ef_launch_count(EfContext* ctx, int64_t* n) {
 // ---------------------------------------------------------------------------------------------------------------
 // named buffers
 // ---------------------------------------------------------------------------------------------------------------
+// pyramid buffer `base` (EF_BUF_VMAP_CURR ..) of a tracker at `level`; n: its level-0 pixels
+static int odom_buffer(const OdomDev& od, int base, int level, size_t n, void** p, size_t* b) {
+  if (level < 0 || level >= NUM_PYRS) return EF_EINVAL;
+  const size_t nl = (size_t)od.rows[level] * od.cols[level];
+  switch (base) {
+    case EF_BUF_VMAP_CURR: *p = od.vmap_curr[level]; *b = nl * 12; break;
+    case EF_BUF_NMAP_CURR: *p = od.nmap_curr[level]; *b = nl * 12; break;
+    case EF_BUF_VMAP_G_PREV: *p = od.vmap_g_prev[level]; *b = nl * 12; break;
+    case EF_BUF_NMAP_G_PREV: *p = od.nmap_g_prev[level]; *b = nl * 12; break;
+    case EF_BUF_LAST_DEPTH: *p = od.lastDepth[level]; *b = nl * 4; break;
+    case EF_BUF_NEXT_DEPTH: *p = od.nextDepth[level]; *b = nl * 4; break;
+    case EF_BUF_LAST_IMAGE: *p = od.lastImage[level]; *b = nl; break;
+    case EF_BUF_NEXT_IMAGE: *p = od.nextImage[level]; *b = nl; break;
+    case EF_BUF_LAST_NEXT_IMAGE: *p = od.lastNextImage[level]; *b = nl; break;
+    case EF_BUF_DIDX: *p = od.dIdx[level]; *b = nl * 2; break;
+    case EF_BUF_DIDY: *p = od.dIdy[level]; *b = nl * 2; break;
+    case EF_BUF_DEPTH_TMP: *p = od.depth_tmp[level]; *b = nl * 2; break;
+    case EF_BUF_CORRES: *p = od.corres[level]; *b = nl * 16; break;
+    case EF_BUF_VMAPS_TMP: *p = od.vmaps_tmp; *b = n * 16; break;
+    default: return EF_EINVAL;
+  }
+  return 0;
+}
+
 extern "C" int ef_buffer(EfContext* ctx, int32_t id, int32_t level, void** dev_ptr, size_t* bytes) {
   if (!ctx) return EF_EINVAL;
   const size_t n = (size_t)ctx->cfg.width * ctx->cfg.height;
@@ -364,27 +390,9 @@ extern "C" int ef_buffer(EfContext* ctx, int32_t id, int32_t level, void** dev_p
       default: return EF_EINVAL;
     }
   } else {
-    const int which = id / 100, base = id % 100;
-    if (which < 0 || which > 1 || level < 0 || level >= NUM_PYRS) return EF_EINVAL;
-    OdomDev& od = ctx->odom[which];
-    const size_t nl = (size_t)od.rows[level] * od.cols[level];
-    switch (base) {
-      case EF_BUF_VMAP_CURR: p = od.vmap_curr[level]; b = nl * 12; break;
-      case EF_BUF_NMAP_CURR: p = od.nmap_curr[level]; b = nl * 12; break;
-      case EF_BUF_VMAP_G_PREV: p = od.vmap_g_prev[level]; b = nl * 12; break;
-      case EF_BUF_NMAP_G_PREV: p = od.nmap_g_prev[level]; b = nl * 12; break;
-      case EF_BUF_LAST_DEPTH: p = od.lastDepth[level]; b = nl * 4; break;
-      case EF_BUF_NEXT_DEPTH: p = od.nextDepth[level]; b = nl * 4; break;
-      case EF_BUF_LAST_IMAGE: p = od.lastImage[level]; b = nl; break;
-      case EF_BUF_NEXT_IMAGE: p = od.nextImage[level]; b = nl; break;
-      case EF_BUF_LAST_NEXT_IMAGE: p = od.lastNextImage[level]; b = nl; break;
-      case EF_BUF_DIDX: p = od.dIdx[level]; b = nl * 2; break;
-      case EF_BUF_DIDY: p = od.dIdy[level]; b = nl * 2; break;
-      case EF_BUF_DEPTH_TMP: p = od.depth_tmp[level]; b = nl * 2; break;
-      case EF_BUF_CORRES: p = od.corres[level]; b = nl * 16; break;
-      case EF_BUF_VMAPS_TMP: p = od.vmaps_tmp; b = n * 16; break;
-      default: return EF_EINVAL;
-    }
+    const int which = id / 100;
+    if (which < 0 || which > 1) return EF_EINVAL;
+    RC(odom_buffer(ctx->odom[which], id % 100, level, n, &p, &b));
   }
   if (dev_ptr) *dev_ptr = p;
   if (bytes) *bytes = b;
@@ -476,7 +484,7 @@ extern "C" int ef_odom_track(EfContext* ctx, int which, double* T_wc, int32_t rg
   RC(upload_gn(ctx, which, offsetof(GNState, T_wc), T_wc, sizeof(double) * 16));
   CU(cudaStreamSynchronize(ctx->stream));
   RC(odom_track_async(ctx, which, rgb_only != 0, icp_weight, pyramid != 0, fast_odom != 0, so3 != 0));
-  RC(odom_finish_async(ctx, which, 1.0f, true));
+  RC(odom_finish_async(ctx, which, 1.0f, true, which == 0 ? ctx->map.pose : nullptr));
   GNState g;
   RC(download_gn(ctx, which, &g));
   memcpy(T_wc, g.T_wc, sizeof(double) * 16);
@@ -730,7 +738,8 @@ extern "C" int ef_map_upload(EfContext* ctx, const float* in12, int32_t count) {
 // ---------------------------------------------------------------------------------------------------------------
 // global-surface render (ef_render.cu)
 // ---------------------------------------------------------------------------------------------------------------
-static bool finite_all(const float* a, int n) {
+template <typename T>
+static bool finite_all(const T* a, int n) {
   for (int i = 0; i < n; ++i)
     if (!isfinite(a[i])) return false;
   return true;
@@ -926,6 +935,92 @@ extern "C" int ef_track_view(EfContext* ctx, const EfTrackView* v, const uint8_t
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// cameras: processFrame for a sensor of the context's map (ef_track.cu, on the camera's own buffers and tracker slot)
+// ---------------------------------------------------------------------------------------------------------------
+// the track view's size rule
+static bool camera_config_ok(const EfCameraConfig* c) {
+  if (!c) return false;
+  const int w = c->width, h = c->height;
+  return w >= 32 && w <= 4096 && h >= 32 && h <= 4096 && isfinite(c->fx) && isfinite(c->fy) && c->fx != 0.f && c->fy != 0.f &&
+         isfinite(c->cx) && isfinite(c->cy) && isfinite(c->depth_cutoff) && c->depth_cutoff > 0.f && isfinite(c->max_depth) &&
+         c->max_depth > 0.f && isfinite(c->conf_threshold) && c->time_delta >= 0 && isfinite(c->icp_weight) && c->icp_weight >= 0.f;
+}
+static bool camera_of(const EfContext* ctx, const EfCamera* cam) {
+  if (!ctx || !cam) return false;
+  for (const EfCamera* c : ctx->cameras)
+    if (c == cam) return true;
+  return false;
+}
+static bool camera_frame_ok(const EfCameraFrame* f) {
+  if (!f || f->time < 0 || !isfinite(f->weight_multiplier) || f->weight_multiplier < 0.f) return false;
+  if (f->has_pose && !finite_all(f->T_wc, 16)) return false;
+  return true;
+}
+// the first frame sets the pose; fuse follows ef_map_fuse_view's rule
+static int camera_frame_state(const EfContext* ctx, const EfCamera* cam, const EfCameraFrame* f) {
+  if (!cam->has_frame && !f->has_pose) return EF_ESTATE;
+  return f->fuse ? fuse_view_state(ctx) : 0;
+}
+
+extern "C" int ef_camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out) {
+  if (!ctx || !out || !camera_config_ok(cfg)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  return camera_create(ctx, cfg, out);
+}
+extern "C" int ef_camera_destroy(EfContext* ctx, EfCamera* cam) {
+  if (!camera_of(ctx, cam)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  camera_destroy(ctx, cam);
+  return 0;
+}
+extern "C" int ef_camera_frame_device(EfContext* ctx, EfCamera* cam, const EfCameraFrame* f, const uint8_t* rgb_dev, const uint16_t* depth_dev,
+                                      EfCameraResult* out_dev) {
+  if (!camera_of(ctx, cam) || !camera_frame_ok(f) || !rgb_dev || !depth_dev || !out_dev || !aligned(depth_dev, 2) || !aligned(out_dev, 8))
+    return EF_EINVAL;
+  RC(camera_frame_state(ctx, cam, f));
+  CU(cudaSetDevice(ctx->device));
+  return camera_frame_async(ctx, cam, f, rgb_dev, depth_dev, false, out_dev);
+}
+extern "C" int ef_camera_frame(EfContext* ctx, EfCamera* cam, const EfCameraFrame* f, const uint8_t* rgb, const uint16_t* depth, EfCameraResult* out,
+                               EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace) {
+  if (!camera_of(ctx, cam) || !camera_frame_ok(f) || !rgb || !depth || !out || max_trace < 0 || (max_trace > 0 && !trace)) return EF_EINVAL;
+  RC(camera_frame_state(ctx, cam, f));
+  CU(cudaSetDevice(ctx->device));
+  RC(camera_frame_async(ctx, cam, f, rgb, depth, true, nullptr));
+  RC(camera_read(ctx, cam, out, trace, max_trace, n_trace));  // (synchronises)
+  return ef_map_count(ctx, &ctx->host_count);
+}
+extern "C" int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32_t level, void** dev_ptr, size_t* bytes) {
+  if (!camera_of(ctx, cam)) return EF_EINVAL;
+  const size_t n = (size_t)cam->cfg.width * cam->cfg.height;
+  void* p = nullptr;
+  size_t b = 0;
+  if (id < 40) {
+    switch (id) {
+      case EF_BUF_RGB: p = cam->rgb; b = n * 3; break;
+      case EF_BUF_RGBA: p = cam->rgba; b = n * 4; break;
+      case EF_BUF_DEPTH_RAW: p = cam->depth_raw; b = n * 2; break;
+      case EF_BUF_DEPTH_FILTERED: p = cam->depth_filtered; b = n * 2; break;
+      case EF_BUF_DEPTH_METRIC: p = cam->target.depth_metric; b = n * 4; break;
+      case EF_BUF_DEPTH_METRIC_FILTERED: p = cam->target.depth_metric_filtered; b = n * 4; break;
+      case EF_BUF_IMAGE: p = cam->image; b = n * 4; break;
+      case EF_BUF_VERTEX: p = cam->vertex; b = n * 16; break;
+      case EF_BUF_NORMAL: p = cam->normal; b = n * 16; break;
+      case EF_BUF_TIME: p = cam->time; b = n * 2; break;
+      case EF_BUF_FILL_IMAGE: p = cam->fill_image; b = n * 4; break;
+      case EF_BUF_FILL_VERTEX: p = cam->fill_vertex; b = n * 16; break;
+      case EF_BUF_FILL_NORMAL: p = cam->fill_normal; b = n * 16; break;
+      default: return EF_EINVAL;
+    }
+  } else {
+    RC(odom_buffer(ctx->odom[cam->slot], id, level, n, &p, &b));
+  }
+  if (dev_ptr) *dev_ptr = p;
+  if (bytes) *bytes = b;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // whole frame
 // ---------------------------------------------------------------------------------------------------------------
 // ElasticFusion::predict, reference Core/ElasticFusion.cpp:621-653 (lost == false, lastFrameRecovery == false)
@@ -1052,7 +1147,7 @@ static int local_loop_async(EfContext* ctx) {
   RC(odom_init_icp_pred(ctx, 1, (const float*)t.vertex, (const float*)t.normal));
   RC(odom_populate(ctx, 1, (const uint8_t*)t.image, od.nextDepth, od.nextImage, true));
   RC(odom_track_async(ctx, 1, false, 10.0f, ctx->pyramid, ctx->fast_odom, false));
-  RC(odom_finish_async(ctx, 1, 1.0f, true));
+  RC(odom_finish_async(ctx, 1, 1.0f, true, nullptr));
   return map_loop_constraints_async(ctx, ctx->cfg.count_thresh, ctx->cfg.err_thresh, ctx->cfg.cov_thresh);
 }
 
@@ -1107,14 +1202,14 @@ static int frame_begin_device(EfContext* ctx, const uint8_t* rgb_dev, const uint
     if (alias)
       for (int i = 0; i < NUM_PYRS; ++i) od.nextDepth[i] = saved[i];
     RC(rc);
-    RC(odom_finish_async(ctx, 0, weight_multiplier, true));
+    RC(odom_finish_async(ctx, 0, weight_multiplier, true, ctx->map.pose));
   } else {
     CU(cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->pin_small->T_wc, in_T_wc, sizeof(double) * 16);
     CU(cudaMemcpyAsync(ctx->dev_small->T_wc, ctx->pin_small->T_wc, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
     ctx->so3_ready = false;  // no tracking for this frame: the SO(3) result of its input side is not used
     RC(odom_set_pose_async(ctx, 0, ctx->dev_small->T_wc));
-    RC(odom_finish_async(ctx, 0, weight_multiplier, false));
+    RC(odom_finish_async(ctx, 0, weight_multiplier, false, ctx->map.pose));
   }
   // (k_gn_finish also refreshed the map kernels' float pose + inverse from the new T_wc)
   ef_stage(ctx, 6);

@@ -16,10 +16,11 @@ constexpr int RED_THREADS = 256;     // threads per reduction CTA
 constexpr int MAX_RED_BLOCKS = 1184; // 8 resident 256-thread CTAs per SM on up to 148 SMs (H100: 132)
 constexpr int PARTIAL_STRIDE = 64;   // floats per CTA partial: [0,29) geometric system, [32,61) photometric system
 constexpr int MAX_TRACE = 48;
-// tracker slots of EfContext::odom: 0 frameToModel, 1 modelToModel (both sized for the context's camera), and the tracker of
-// ef_track_view*, whose buffers are sized for the largest view so far
-constexpr int NUM_TRACKERS = 3;
+// tracker slots of EfContext::odom: 0 frameToModel, 1 modelToModel (both sized for the context's camera), the tracker of
+// ef_track_view*, whose buffers are sized for the largest view so far, and one per live EfCamera, sized for its camera
 constexpr int VIEW_TRACKER = 2;
+constexpr int CAMERA_TRACKER0 = 3;
+constexpr int NUM_TRACKERS = CAMERA_TRACKER0 + EF_MAX_CAMERAS;
 constexpr int DENSE_FACTOR = 20;  // ElasticFusion::denseEnough decimates the predicted image by 20 (ElasticFusion.cpp:258)
 
 // ElasticFusion::denseEnough (ElasticFusion.cpp:256-268) from the number of lit samples of the decimated image
@@ -330,6 +331,24 @@ struct MapTarget {
   ScanTiles* scan;  // covers the clean's capacity + W*H surfels and fuse's W*H pixels
 };
 
+// What combinedPredict at a device pose record writes for a camera of its own (ef_camera_frame*): the model view (any output may be
+// null), the lit samples of its decimation (null: not counted) and, fill_vertex given, the fill-in of predict() from the camera's
+// filtered depth and RGB in the same pass (ElasticFusion.cpp:621-653)
+struct PredictTarget {
+  int rows, cols;
+  float cx, cy, fx, fy;
+  const MapPose* pose;
+  uchar4* image;
+  float4 *vertex, *normal;
+  uint16_t* time;
+  int* dense_count;
+  const uint16_t* fill_depth;  // W*H filtered millimetres
+  const uint8_t* fill_rgb;     // W*H*3
+  int fill_pass_img;           // frameToFrameRGB: the fill-in image is the live RGB everywhere
+  uchar4* fill_image;
+  float4 *fill_vertex, *fill_normal;
+};
+
 }  // namespace ef
 
 struct EfContext {
@@ -353,6 +372,8 @@ struct EfContext {
 
   ef::OdomDev odom[ef::NUM_TRACKERS];
   float odom_cam[ef::NUM_TRACKERS][4];  // level-0 {fx, fy, cx, cy} of tracker w: the host's copy of what its GNState holds
+  ef::ScanTiles* odom_tiles[ef::NUM_TRACKERS];  // tile states of tracker w's candidate compaction (null: the context's own)
+  EfCamera* cameras[EF_MAX_CAMERAS];           // live cameras, by tracker slot (CAMERA_TRACKER0 + i)
   ef::MapDev map;
   ef::Textures tex;
   ef::Lookahead la;
@@ -387,6 +408,30 @@ struct EfContext {
                      // first call and grown with the view
   cudaEvent_t view_pose_sent;  // ctx->stream: the last view's pose and weighting have been copied out of PinStaging
   ef::Arena arena;   // every device buffer of the context
+};
+
+// A camera of a context (ef_camera_*): its tracker slot, inputs, prediction, fill-in and map-write buffers, all at its own size
+struct EfCamera {
+  int slot;                // tracker slot in ctx->odom (CAMERA_TRACKER0 + its index in ctx->cameras)
+  EfCameraConfig cfg;
+  bool has_frame;          // a first frame has set its pose and previous intensity pyramid
+  ef::Arena arena;         // every device buffer below and those of ctx->odom[slot]
+  uint8_t *rgb, *rgba;     // its inputs (rgb and depth_raw are the map target's, which fuse reads)
+  uint16_t *depth_raw, *depth_filtered;
+  uchar4* image;           // predict(): the model its next frame tracks against, and the fill-in
+  float4 *vertex, *normal;
+  uint16_t* time;
+  uchar4* fill_image;
+  float4 *fill_vertex, *fill_normal;
+  int* dense_count;        // lit samples of the prediction's decimation
+  ef::ScanTiles scan;      // look-back tile states of its candidate compaction
+  ef::MapPose* pose;       // its pose record, written by k_gn_finish
+  ef::MapTarget target;    // its map-write side (pose record and tracker weighting set)
+  void* target_state;      // map_camera_target's
+  EfCameraResult* result;  // device: the result of its last frame (the host call reads it back)
+  double* pin_T;           // pinned staging of a frame's has_pose T_wc, rewritten after pose_sent
+  double* dev_T;
+  cudaEvent_t pose_sent;
 };
 
 // error propagation of the host entry points: a CUDA error code, or the code of a failed internal call
@@ -487,12 +532,21 @@ int track_view_async(EfContext* ctx, const EfTrackView* v, const uint8_t* rgb, c
 // the view tracker's GNState and the view's dense-sample count into host memory (synchronises)
 int track_view_read(EfContext* ctx, GNState* g, int* lit);
 void track_view_free(EfContext* ctx);
+// ef_camera_* (include/efusion_b200.h): a camera's buffers and tracker slot (EF_ENOMEM / EF_ESTATE as the ABI says); one camera frame
+// (host inputs when from_host, the result into out_dev when given, else into the camera's own result); that own result and the trace
+// of its last frame (synchronises); and its release
+int camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out);
+int camera_frame_async(EfContext* ctx, EfCamera* cam, const EfCameraFrame* f, const uint8_t* rgb, const uint16_t* depth, bool from_host,
+                       EfCameraResult* out_dev);
+int camera_read(EfContext* ctx, EfCamera* cam, EfCameraResult* out, EfSolveTrace* trace, int max_trace, int* n_trace);
+void camera_destroy(EfContext* ctx, EfCamera* cam);
 
 // ef_reduce.cu: SO(3) loop, Gauss-Newton schedule and the stage API's reductions
 int odom_cluster_size(int want);
 int odom_so3_async(EfContext* ctx, int which);
 int odom_track_async(EfContext* ctx, int which, bool rgbOnly, float icpWeight, bool pyramid, bool fastOdom, bool so3);
-int odom_finish_async(EfContext* ctx, int which, float weightMultiplier, bool have_track);
+// pose_record: the map pose record the finished pose is written to as well (null: none)
+int odom_finish_async(EfContext* ctx, int which, float weightMultiplier, bool have_track, MapPose* pose_record);
 int odom_set_pose_async(EfContext* ctx, int which, const double* T_dev);
 int launch_se3_step_raw(EfContext* ctx, int which, int level, bool do_icp, bool do_rgb, float sigma);
 int launch_rgb_residual_raw(EfContext* ctx, int which, int level);
@@ -523,6 +577,11 @@ MapTarget map_frame_target(EfContext* ctx);
 // a fuse view's buffers, grown to the view (EF_ENOMEM if they cannot be: the context stays usable), with its pose and weighting
 // staged and uploaded to MapDev::view_pose; rgb / depth_raw: where its inputs may be uploaded (W*H*3, W*H)
 int map_fuse_view_target(EfContext* ctx, const EfFuseView* view, MapTarget* out, uint8_t** rgb, uint16_t** depth_raw);
+// a camera's own map-write buffers, as a fuse view's of its size, from `arena` (ef_camera_*): its inputs, index map and scratch. pose and
+// weighting are left to the caller; *state keeps the index state and tile states the target points to (map_camera_target_free)
+int map_camera_target(EfContext* ctx, Arena& arena, int rows, int cols, float fx, float fy, float cx, float cy, void** state, MapTarget* out,
+                      uint8_t** rgb, uint16_t** depth_raw);
+void map_camera_target_free(void* state);
 int map_predict_indices_async(EfContext* ctx, const MapTarget& t, int time, float max_depth, int time_delta, int vis_mode = 0);
 // the textures of a frame's index pass that no clean has written yet (nothing to do otherwise)
 int map_index_textures_async(EfContext* ctx, const MapTarget& t);
@@ -540,6 +599,8 @@ int map_fill_in_async(EfContext* ctx, bool passthrough_geometry, bool passthroug
 // dense_count: where the lit samples of the predicted image's decimation are counted (null: not counted)
 int map_predict_view_async(EfContext* ctx, const EfModelView* view, uint8_t* image4, float* vertex4, float* normal4, uint16_t* time,
                            int* dense_count = nullptr);
+// the same at t.pose (device), writing t's outputs, dense count and fill-in
+int map_predict_target_async(EfContext* ctx, const PredictTarget& t, float max_depth, float conf_threshold, int time, int max_time, int time_delta);
 int map_dense_enough_async(EfContext* ctx);
 int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
 int map_loop_reset_async(EfContext* ctx);

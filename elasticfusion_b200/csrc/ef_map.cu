@@ -1837,31 +1837,57 @@ static int stage_view_pose(EfContext* ctx, const double* T_wc, float weighting) 
   return 0;
 }
 
-// the raycast above at the view's own pose, camera and size, on the off-frame z-buffer, with no fill-in; the dense count only
-// when asked for (a track view's)
-int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time, int* dense_count) {
+// the raycast above at a camera of its own and the pose record `pose`, on the off-frame z-buffer; f: its dense count and fill-in
+static int predict_offframe(EfContext* ctx, const RayArgs& a, const MapPose* pose, uchar4* image, float4* vertex, float4* normal, uint16_t* time,
+                            const FillOut& f) {
   MapDev& m = ctx->map;
-  const size_t n = (size_t)v->width * v->height;
+  const size_t n = (size_t)a.rows * a.cols;
   unsigned long long* zbuf = nullptr;
   RC(offframe_zbuf(ctx, n, &zbuf));
-  RC(stage_view_pose(ctx, v->T_wc, -1.0f));
-  RayArgs a;
-  a.rows = v->height;
-  a.cols = v->width;
-  a.c = Cam{v->cx, v->cy, v->fx, v->fy};
-  a.max_depth = v->max_depth;
-  a.conf_threshold = v->conf_threshold;
-  a.time = v->time;
-  a.max_time = v->max_time;
-  a.time_delta = v->time_delta;
-  EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, m.count, zbuf,
-            dense_count);
-  FillOut f = {};
-  f.dense_count = dense_count;
-  EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, m.view_pose, m.pos_conf, m.color_time, m.norm_rad, zbuf,
-            reinterpret_cast<uchar4*>(image), reinterpret_cast<float4*>(vertex), reinterpret_cast<float4*>(normal), time, (float*)nullptr, f);
+  EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, pose, m.pos_conf, m.color_time, m.norm_rad, m.count, zbuf, f.dense_count);
+  EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, pose, m.pos_conf, m.color_time, m.norm_rad, zbuf, image, vertex, normal, time,
+            (float*)nullptr, f);
   CHECK_LAST();
   return 0;
+}
+
+static RayArgs ray_args(int rows, int cols, const Cam& c, float max_depth, float conf_threshold, int time, int max_time, int time_delta) {
+  RayArgs a;
+  a.rows = rows;
+  a.cols = cols;
+  a.c = c;
+  a.max_depth = max_depth;
+  a.conf_threshold = conf_threshold;
+  a.time = time;
+  a.max_time = max_time;
+  a.time_delta = time_delta;
+  return a;
+}
+
+// at the view's own pose, camera and size, with no fill-in; the dense count only when asked for (a track view's)
+int map_predict_view_async(EfContext* ctx, const EfModelView* v, uint8_t* image, float* vertex, float* normal, uint16_t* time, int* dense_count) {
+  RC(stage_view_pose(ctx, v->T_wc, -1.0f));
+  FillOut f = {};
+  f.dense_count = dense_count;
+  return predict_offframe(ctx, ray_args(v->height, v->width, Cam{v->cx, v->cy, v->fx, v->fy}, v->max_depth, v->conf_threshold, v->time,
+                                        v->max_time, v->time_delta),
+                          ctx->map.view_pose, reinterpret_cast<uchar4*>(image), reinterpret_cast<float4*>(vertex),
+                          reinterpret_cast<float4*>(normal), time, f);
+}
+
+int map_predict_target_async(EfContext* ctx, const PredictTarget& t, float max_depth, float conf_threshold, int time, int max_time, int time_delta) {
+  FillOut f = {};
+  f.dense_count = t.dense_count;
+  if (t.fill_vertex) {
+    f.raw_depth = t.fill_depth;
+    f.rgb = t.fill_rgb;
+    f.pass_img = t.fill_pass_img;
+    f.vertex = t.fill_vertex;
+    f.normal = t.fill_normal;
+    f.image = t.fill_image;
+  }
+  return predict_offframe(ctx, ray_args(t.rows, t.cols, Cam{t.cx, t.cy, t.fx, t.fy}, max_depth, conf_threshold, time, max_time, time_delta),
+                          t.pose, t.image, t.vertex, t.normal, t.time, f);
 }
 
 // ---- fuse view (ef_map_fuse_view*): its own inputs, index map and scratch, in one allocation grown to the largest view ----
@@ -1915,53 +1941,38 @@ static size_t fuse_view_layout(FuseViewBuffers& V, uint8_t* base, size_t px, siz
   return off;
 }
 
-int map_fuse_view_target(EfContext* ctx, const EfFuseView* v, MapTarget* out, uint8_t** rgb, uint16_t** depth_raw) {
-  if (!ctx->fuse_view) {
-    FuseViewBuffers* nv = new (std::nothrow) FuseViewBuffers();
-    if (!nv) return EF_ENOMEM;
-    ctx->fuse_view = nv;
-  }
-  FuseViewBuffers& V = *static_cast<FuseViewBuffers*>(ctx->fuse_view);
-  const size_t px = (size_t)v->width * v->height, cap = (size_t)ctx->map.capacity;
-  if (px > V.px) {
-    CU(cudaStreamSynchronize(ctx->stream));  // the previous view may still read the old block
-    if (V.block) CU(cudaFree(V.block));
-    V.block = nullptr;
-    V.px = 0;
-    const size_t bytes = fuse_view_layout(V, nullptr, px, cap);
-    if (cudaMalloc(&V.block, bytes) != cudaSuccess) {
-      V.block = nullptr;
-      cudaGetLastError();  // (an allocation failure is not sticky: the context stays usable)
-      return EF_ENOMEM;
-    }
-    fuse_view_layout(V, (uint8_t*)V.block, px, cap);
-    V.px = px;
-    // every key stale, no new surfels, clean's dispenser and tickets at zero and no first mover, no published tile state
-    CU(cudaMemsetAsync(V.index_keys, 0xff, px * sizeof(unsigned long long), ctx->stream));
-    CU(cudaMemsetAsync(V.new_count, 0, 4, ctx->stream));
-    CU(cudaMemsetAsync(V.clean_ctl, 0, 8, ctx->stream));
-    CU(cudaMemsetAsync(V.clean_ctl + 2, 0xff, 8, ctx->stream));
-    CU(cudaMemsetAsync(V.scan.counter, 0, 8, ctx->stream));
-    CU(cudaMemsetAsync(V.scan.state, 0, V.scan.bytes, ctx->stream));
-    V.scan.epoch = 0;
-    V.ix.pass = 0;
-    V.ix.keys_only = false;
-    V.ix.vis_pending = false;
-  }
-  RC(stage_view_pose(ctx, v->T_wc, v->weighting));
+// the buffers of a px-pixel view in `block` (fuse_view_layout's bytes), as a fresh view finds them: every key stale, no new surfels,
+// clean's dispenser and tickets at zero and no first mover, no published tile state
+static int arm_view_buffers(EfContext* ctx, FuseViewBuffers& V, void* block, size_t px) {
+  V.block = block;
+  fuse_view_layout(V, (uint8_t*)block, px, (size_t)ctx->map.capacity);
+  V.px = px;
+  CU(cudaMemsetAsync(V.index_keys, 0xff, px * sizeof(unsigned long long), ctx->stream));
+  CU(cudaMemsetAsync(V.new_count, 0, 4, ctx->stream));
+  CU(cudaMemsetAsync(V.clean_ctl, 0, 8, ctx->stream));
+  CU(cudaMemsetAsync(V.clean_ctl + 2, 0xff, 8, ctx->stream));
+  CU(cudaMemsetAsync(V.scan.counter, 0, 8, ctx->stream));
+  CU(cudaMemsetAsync(V.scan.state, 0, V.scan.bytes, ctx->stream));
+  V.scan.epoch = 0;
+  V.ix.pass = 0;
+  V.ix.keys_only = false;
+  V.ix.vis_pending = false;
+  return 0;
+}
+
+// the target of a rows x cols view on V's buffers; its pose record and weighting are the caller's to set
+static MapTarget view_target(FuseViewBuffers& V, int rows, int cols, float fx, float fy, float cx, float cy) {
   MapTarget t = {};
-  t.rows = v->height;
-  t.cols = v->width;
-  t.cx = v->cx;
-  t.cy = v->cy;
-  t.fx = v->fx;
-  t.fy = v->fy;
+  t.rows = rows;
+  t.cols = cols;
+  t.cx = cx;
+  t.cy = cy;
+  t.fx = fx;
+  t.fy = fy;
   t.rgb = V.rgb;
   t.depth_metric = V.depth_metric;
   t.depth_metric_filtered = V.depth_metric_filtered;
   t.synth_depth = nullptr;
-  t.pose = ctx->map.view_pose;
-  t.weighting = &ctx->dev_small->view_weighting;
   t.index_keys = V.index_keys;
   t.key_texels = V.px;
   t.index = V.index;
@@ -1978,11 +1989,55 @@ int map_fuse_view_target(EfContext* ctx, const EfFuseView* v, MapTarget* out, ui
   t.clean_ctl = V.clean_ctl;
   t.clean_total = V.clean_total;
   t.scan = &V.scan;
+  return t;
+}
+
+int map_fuse_view_target(EfContext* ctx, const EfFuseView* v, MapTarget* out, uint8_t** rgb, uint16_t** depth_raw) {
+  if (!ctx->fuse_view) {
+    FuseViewBuffers* nv = new (std::nothrow) FuseViewBuffers();
+    if (!nv) return EF_ENOMEM;
+    ctx->fuse_view = nv;
+  }
+  FuseViewBuffers& V = *static_cast<FuseViewBuffers*>(ctx->fuse_view);
+  const size_t px = (size_t)v->width * v->height;
+  if (px > V.px) {
+    CU(cudaStreamSynchronize(ctx->stream));  // the previous view may still read the old block
+    if (V.block) CU(cudaFree(V.block));
+    V.block = nullptr;
+    V.px = 0;
+    void* block = nullptr;
+    if (cudaMalloc(&block, fuse_view_layout(V, nullptr, px, (size_t)ctx->map.capacity)) != cudaSuccess) {
+      cudaGetLastError();  // (an allocation failure is not sticky: the context stays usable)
+      return EF_ENOMEM;
+    }
+    RC(arm_view_buffers(ctx, V, block, px));
+  }
+  RC(stage_view_pose(ctx, v->T_wc, v->weighting));
+  MapTarget t = view_target(V, v->height, v->width, v->fx, v->fy, v->cx, v->cy);
+  t.pose = ctx->map.view_pose;
+  t.weighting = &ctx->dev_small->view_weighting;
   *out = t;
   *rgb = V.rgb;
   *depth_raw = V.depth_raw;
   return 0;
 }
+
+int map_camera_target(EfContext* ctx, Arena& arena, int rows, int cols, float fx, float fy, float cx, float cy, void** state, MapTarget* out,
+                      uint8_t** rgb, uint16_t** depth_raw) {
+  FuseViewBuffers* V = new (std::nothrow) FuseViewBuffers();
+  if (!V) return EF_ENOMEM;
+  *state = V;
+  const size_t px = (size_t)rows * cols;
+  uint8_t* block = nullptr;
+  CU(arena_alloc(ctx, arena, &block, fuse_view_layout(*V, nullptr, px, (size_t)ctx->map.capacity)));
+  RC(arm_view_buffers(ctx, *V, block, px));
+  *out = view_target(*V, rows, cols, fx, fy, cx, cy);
+  *rgb = V->rgb;
+  *depth_raw = V->depth_raw;
+  return 0;
+}
+
+void map_camera_target_free(void* state) { delete static_cast<FuseViewBuffers*>(state); }
 
 void map_fuse_view_free(EfContext* ctx) {
   FuseViewBuffers* V = static_cast<FuseViewBuffers*>(ctx->fuse_view);

@@ -17,6 +17,7 @@
 #include <string.h>
 
 #include <new>
+#include <utility>
 
 #include "ef_device.cuh"
 #include "ef_dmath.cuh"
@@ -491,13 +492,9 @@ __global__ void k_track_view_reset(GNState* gn, const double* __restrict__ T_wc,
   for (int k = 0; k < 16; ++k) gn->T_wc[k] = T_wc[k];
 }
 
-// EfTrackResult of a track view (ef_track_view_device): pose, RGBDOdometry's public results, getCovariance and denseEnough
-__global__ void k_track_view_result(const GNState* __restrict__ gn, const int* __restrict__ dense_count, int rows, int cols,
-                                    EfTrackResult* __restrict__ out) {
-  pdl_enter();
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  for (int k = 0; k < 16; ++k) out->T_wc[k] = gn->T_wc[k];
-  EfOdomStats& s = out->stats;
+// pose, RGBDOdometry's public results and getCovariance of a tracker
+__device__ __forceinline__ void odom_result(const GNState* __restrict__ gn, double* T_wc, EfOdomStats& s, double* covariance) {
+  for (int k = 0; k < 16; ++k) T_wc[k] = gn->T_wc[k];
   s.lastICPError = gn->lastICPError;
   s.lastICPCount = gn->lastICPCount;
   s.lastRGBError = gn->lastRGBError;
@@ -506,8 +503,27 @@ __global__ void k_track_view_result(const GNState* __restrict__ gn, const int* _
   s.lastSO3Count = gn->lastSO3Count;
   for (int k = 0; k < 36; ++k) s.lastA[k] = gn->lastA[k];
   for (int k = 0; k < 6; ++k) s.lastb[k] = gn->lastb[k];
-  efm::inv_n<6>(gn->lastA, out->covariance);  // lastA.lu().inverse(), as ef_odom_covariance
+  efm::inv_n<6>(gn->lastA, covariance);  // lastA.lu().inverse(), as ef_odom_covariance
+}
+
+// EfTrackResult of a track view (ef_track_view_device): pose, RGBDOdometry's public results, getCovariance and denseEnough
+__global__ void k_track_view_result(const GNState* __restrict__ gn, const int* __restrict__ dense_count, int rows, int cols,
+                                    EfTrackResult* __restrict__ out) {
+  pdl_enter();
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  odom_result(gn, out->T_wc, out->stats, out->covariance);
   out->dense_enough = dense_enough_of(*dense_count, rows, cols) ? 1 : 0;
+}
+
+// EfCameraResult of a camera frame: the above, whether it tracked, denseEnough of the prediction it tracked against and the weighting
+__global__ void k_camera_result(const GNState* __restrict__ gn, const int* __restrict__ dense_count, int rows, int cols, int tracked,
+                                EfCameraResult* __restrict__ out) {
+  pdl_enter();
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  odom_result(gn, out->T_wc, out->stats, out->covariance);
+  out->tracked = tracked;
+  out->dense_enough = dense_enough_of(*dense_count, rows, cols) ? 1 : 0;
+  out->weighting = gn->weighting;
 }
 
 // =============================================================================================
@@ -520,8 +536,6 @@ inline dim3 grid2d(int cols, int rows) { return dim3((cols + 31) / 32, (rows + 7
 }  // namespace
 
 namespace ef {
-
-static int view_scan_slot(EfContext* ctx, ScanSlot* out);
 
 int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff) {
   OdomDev& od = ctx->odom[which];
@@ -644,12 +658,75 @@ int launch_sobel(EfContext* ctx, int which) {
   }
   a.start[NUM_PYRS] = od.level_start[NUM_PYRS];
   ScanSlot sc;
-  RC(which == VIEW_TRACKER ? view_scan_slot(ctx, &sc) : scan_slot(ctx, &sc));
+  ScanTiles* tiles = ctx->odom_tiles[which];
+  RC(tiles ? scan_slot(ctx, *tiles, &sc) : scan_slot(ctx, &sc));
   EF_LAUNCH(ctx, k_sobel_cand, wave_blocks(ctx, (size_t)od.level_start[NUM_PYRS], 8, SC_THREADS), SC_THREADS, 0, a, od.cand, od.gn, sc.state,
             sc.counter, sc.epoch);
   ctx->maps_dirty[which] = true;  // k_iter1 / k_iter2 read the list ahead of their dependency wait: fence before the next one
   CHECK_LAST();
   return 0;
+}
+
+// ---- one launch sequence for the trackers outside the frame: the track view's and the cameras' -------------------------------
+// A tracker's input buffers at its camera's size
+struct LiveBuffers {
+  uint8_t *rgb, *rgba;  // W*H*3, W*H*4
+  uint16_t *depth_raw, *depth_filtered;
+  float *depth_metric, *depth_metric_filtered;  // null: not computed
+};
+
+// The live side of a frame at tracker `which`'s camera (ElasticFusion.cpp:278-285, initICP and initRGB's intensity half): the inputs
+// copied into b.rgb / b.depth_raw when copy is set (rgb and depth then point there), RGBA, the bilateral filter and metric depths,
+// the depth pyramid with its vertex / normal maps at max_depth, and the intensity pyramid (nextImage)
+static int track_live_side(EfContext* ctx, int which, const LiveBuffers& b, const uint8_t*& rgb, const uint16_t*& depth, bool copy,
+                           cudaMemcpyKind kind, float depth_cutoff, float max_depth) {
+  OdomDev& od = ctx->odom[which];
+  const int w = od.width, h = od.height;
+  const size_t n = (size_t)w * h;
+  if (copy) {
+    CU(cudaMemcpyAsync(b.rgb, rgb, n * 3, kind, ctx->stream));
+    CU(cudaMemcpyAsync(b.depth_raw, depth, n * 2, kind, ctx->stream));
+    rgb = b.rgb;
+    depth = b.depth_raw;
+  }
+  RC(rgb_to_rgba(ctx, h, w, rgb, b.rgba));
+  RC(preprocess_depth(ctx, h, w, depth, depth_cutoff, b.depth_filtered, b.depth_metric, b.depth_metric_filtered));
+  RC(odom_init_icp_depth(ctx, which, b.depth_filtered, max_depth));
+  return odom_populate(ctx, which, b.rgba, nullptr, od.nextImage, false);
+}
+
+// The model side: the predicted maps (A) or, when dense_count is given and not dense enough, the fill-in (B); the image B also when
+// frame_to_frame_rgb. initRGB's depth half is the model's (quirk A.2: it reads the vmaps_tmp initICPModel just filled), aliased to it
+// unless frame_to_frame_rgb builds it from rgba as the frame does.
+struct ModelInputs {
+  const float4 *vtxA, *nrmA, *vtxB, *nrmB;
+  const uchar4 *imgA, *imgB;
+  const int* dense_count;
+  bool frame_to_frame_rgb;
+  const uint8_t* rgba;
+};
+
+// initICPModel + initRGBModel, initRGB's depth half, getIncrementalTransformation and its finish with the velocity weighting
+// (ElasticFusion.cpp:302-383) in tracker `which`, whose pose is the starting point; the finished pose also into pose_record
+static int track_solve(EfContext* ctx, int which, const ModelInputs& m, bool rgb_only, float icp_weight, bool pyramid, bool fast_odom, bool so3,
+                       float weight_multiplier, MapPose* pose_record) {
+  OdomDev& od = ctx->odom[which];
+  RC(odom_model_inputs(ctx, which, m.vtxA, m.nrmA, m.vtxB, m.nrmB, m.imgA, m.imgB, m.dense_count, m.frame_to_frame_rgb ? 1 : 0));
+  float* saved[NUM_PYRS];
+  const bool alias = !m.frame_to_frame_rgb;
+  if (alias) {
+    for (int i = 0; i < NUM_PYRS; ++i) {
+      saved[i] = od.nextDepth[i];
+      od.nextDepth[i] = od.lastDepth[i];
+    }
+  } else {
+    RC(odom_populate(ctx, which, m.rgba, od.nextDepth, od.nextImage, true, false));
+  }
+  const int rc = odom_track_async(ctx, which, rgb_only, icp_weight, pyramid, fast_odom, so3);
+  if (alias)
+    for (int i = 0; i < NUM_PYRS; ++i) od.nextDepth[i] = saved[i];
+  RC(rc);
+  return odom_finish_async(ctx, which, weight_multiplier, true, pose_record);
 }
 
 // ---- track view (ef_track_view*): the frame's tracking recipe at any camera, in tracker slot VIEW_TRACKER --------------------
@@ -668,7 +745,16 @@ struct TrackViewBuffers {
 
 static TrackViewBuffers& tvb(EfContext* ctx) { return *static_cast<TrackViewBuffers*>(ctx->track_view); }
 
-static int view_scan_slot(EfContext* ctx, ScanSlot* out) { return scan_slot(ctx, tvb(ctx).scan, out); }
+// look-back tile states of k_sobel_cand for tracker `which`'s pyramid, from `arena`, and routed to its launches
+static int alloc_cand_tiles(EfContext* ctx, Arena& arena, int which, ScanTiles& scan) {
+  const size_t tiles = (size_t)(ctx->odom[which].level_start[NUM_PYRS] + SC_THREADS - 1) / SC_THREADS + 2;
+  CU(arena_alloc(ctx, arena, &scan.state, tiles, 0));
+  CU(arena_alloc(ctx, arena, &scan.counter, 4, 0));
+  scan.bytes = tiles * 8;
+  scan.epoch = 0;
+  ctx->odom_tiles[which] = &scan;
+  return 0;
+}
 
 static int track_view_alloc(EfContext* ctx, TrackViewBuffers& V, int W, int H) {
   const size_t px = (size_t)W * H;
@@ -681,11 +767,7 @@ static int track_view_alloc(EfContext* ctx, TrackViewBuffers& V, int W, int H) {
   CU(arena_alloc(ctx, V.arena, &V.vertex, px));
   CU(arena_alloc(ctx, V.arena, &V.normal, px));
   CU(arena_alloc(ctx, V.arena, &V.dense_count, 1, 0));
-  const size_t tiles = (size_t)(ctx->odom[VIEW_TRACKER].level_start[NUM_PYRS] + 255) / 256 + 2;  // k_sobel_cand's SC_THREADS-pixel tiles
-  CU(arena_alloc(ctx, V.arena, &V.scan.state, tiles, 0));
-  CU(arena_alloc(ctx, V.arena, &V.scan.counter, 4, 0));
-  V.scan.bytes = tiles * 8;
-  V.scan.epoch = 0;
+  RC(alloc_cand_tiles(ctx, V.arena, VIEW_TRACKER, V.scan));
   CU(cudaStreamSynchronize(ctx->stream));
   V.width = W;
   V.height = H;
@@ -735,33 +817,14 @@ int track_view_async(EfContext* ctx, const EfTrackView* v, const uint8_t* rgb, c
   }
   const float cam[4] = {mv.fx, mv.fy, mv.cx, mv.cy};
   memcpy(ctx->odom_cam[VIEW_TRACKER], cam, sizeof(cam));
-  const size_t n = (size_t)w * h;
-  if (from_host) {
-    CU(cudaMemcpyAsync(V.rgb, rgb, n * 3, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(V.depth_raw, depth, n * 2, cudaMemcpyHostToDevice, ctx->stream));
-    rgb = V.rgb;
-    depth = V.depth_raw;
-  }
-  // live side: initICP(filtered depth, maxDepthProcessed) and initRGB's intensity pyramid
-  RC(rgb_to_rgba(ctx, h, w, rgb, V.rgba));
-  RC(preprocess_depth(ctx, h, w, depth, v->depth_cutoff, V.depth_filtered, nullptr, nullptr));
-  RC(odom_init_icp_depth(ctx, VIEW_TRACKER, V.depth_filtered, mv.max_depth));
-  RC(odom_populate(ctx, VIEW_TRACKER, V.rgba, nullptr, od.nextImage, false));
-  // model side: combinedPredict at the guess (which stages the guess as the view pose), then initICPModel + initRGBModel
+  const LiveBuffers live = {V.rgb, V.rgba, V.depth_raw, V.depth_filtered, nullptr, nullptr};
+  RC(track_live_side(ctx, VIEW_TRACKER, live, rgb, depth, from_host, cudaMemcpyHostToDevice, v->depth_cutoff, mv.max_depth));
+  // model side: combinedPredict at the guess (which stages the guess as the view pose), the tracker reset to it, then the solve
   RC(map_predict_view_async(ctx, &mv, reinterpret_cast<uint8_t*>(V.image), reinterpret_cast<float*>(V.vertex),
                             reinterpret_cast<float*>(V.normal), nullptr, V.dense_count));
   EF_LAUNCH(ctx, k_track_view_reset, 1, 32, 0, od.gn, (const double*)ctx->dev_small->view_pose, w, h, mv.fx, mv.fy, mv.cx, mv.cy);
-  RC(odom_model_inputs(ctx, VIEW_TRACKER, V.vertex, V.normal, V.vertex, V.normal, V.image, V.image, nullptr, 0));
-  // nextDepth = lastDepth, as in the frame (quirk A.2: initRGB's depth half reads the vmaps_tmp initICPModel just filled)
-  float* saved[NUM_PYRS];
-  for (int i = 0; i < NUM_PYRS; ++i) {
-    saved[i] = od.nextDepth[i];
-    od.nextDepth[i] = od.lastDepth[i];
-  }
-  const int rc = odom_track_async(ctx, VIEW_TRACKER, v->rgb_only != 0, v->icp_weight, v->pyramid != 0, v->fast_odom != 0, false);
-  for (int i = 0; i < NUM_PYRS; ++i) od.nextDepth[i] = saved[i];
-  RC(rc);
-  RC(odom_finish_async(ctx, VIEW_TRACKER, 1.0f, true));
+  const ModelInputs m = {V.vertex, V.normal, V.vertex, V.normal, V.image, V.image, nullptr, false, V.rgba};
+  RC(track_solve(ctx, VIEW_TRACKER, m, v->rgb_only != 0, v->icp_weight, v->pyramid != 0, v->fast_odom != 0, false, 1.0f, nullptr));
   if (out_dev) EF_LAUNCH(ctx, k_track_view_result, 1, 32, 0, (const GNState*)od.gn, (const int*)V.dense_count, h, w, out_dev);
   CHECK_LAST();
   return 0;
@@ -780,6 +843,156 @@ void track_view_free(EfContext* ctx) {
   V->arena.release();
   delete V;
   ctx->track_view = nullptr;
+  ctx->odom_tiles[VIEW_TRACKER] = nullptr;
+}
+
+// ---- cameras (ef_camera_*): processFrame for a sensor of its own, in tracker slot cam->slot ----------------------------------
+static int camera_alloc(EfContext* ctx, EfCamera& c) {
+  const EfCameraConfig& k = c.cfg;
+  const size_t px = (size_t)k.width * k.height;
+  RC(alloc_odom(ctx, c.arena, c.slot, k.width, k.height, k.fx, k.fy, k.cx, k.cy));
+  RC(alloc_cand_tiles(ctx, c.arena, c.slot, c.scan));
+  CU(arena_alloc(ctx, c.arena, &c.rgba, px * 4, 0));
+  CU(arena_alloc(ctx, c.arena, &c.depth_filtered, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.image, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.vertex, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.normal, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.time, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.fill_image, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.fill_vertex, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.fill_normal, px, 0));
+  CU(arena_alloc(ctx, c.arena, &c.dense_count, 1, 0));
+  CU(arena_alloc(ctx, c.arena, &c.pose, 1, 0));
+  CU(arena_alloc(ctx, c.arena, &c.result, 1, 0));
+  CU(arena_alloc(ctx, c.arena, &c.dev_T, 16, 0));
+  RC(map_camera_target(ctx, c.arena, k.height, k.width, k.fx, k.fy, k.cx, k.cy, &c.target_state, &c.target, &c.rgb, &c.depth_raw));
+  c.target.pose = c.pose;
+  c.target.weighting = &ctx->odom[c.slot].gn->weighting;
+  unsigned long long* zbuf = nullptr;
+  RC(offframe_zbuf(ctx, px, &zbuf));  // grown here, so that a frame never allocates
+  CU(cudaMallocHost((void**)&c.pin_T, sizeof(double) * 16));
+  CU(cudaEventCreateWithFlags(&c.pose_sent, cudaEventDisableTiming));
+  CU(cudaEventRecord(c.pose_sent, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+// everything of a camera, allocated or not
+static void camera_release(EfContext* ctx, EfCamera* c) {
+  cudaStreamSynchronize(ctx->stream);
+  c->arena.release();
+  if (c->target_state) map_camera_target_free(c->target_state);
+  if (c->pin_T) cudaFreeHost(c->pin_T);
+  if (c->pose_sent) cudaEventDestroy(c->pose_sent);
+  memset(&ctx->odom[c->slot], 0, sizeof(OdomDev));
+  ctx->odom_tiles[c->slot] = nullptr;
+  delete c;
+}
+
+int camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out) {
+  int i = 0;
+  while (i < EF_MAX_CAMERAS && ctx->cameras[i]) ++i;
+  if (i == EF_MAX_CAMERAS) return EF_ESTATE;
+  EfCamera* c = new (std::nothrow) EfCamera();
+  if (!c) return EF_ENOMEM;
+  c->slot = CAMERA_TRACKER0 + i;
+  c->cfg = *cfg;
+  if (int rc = camera_alloc(ctx, *c)) {
+    camera_release(ctx, c);
+    if (rc != (int)cudaErrorMemoryAllocation && rc != EF_ENOMEM) return rc;
+    cudaGetLastError();  // (an allocation failure is not sticky: the context stays usable)
+    return EF_ENOMEM;
+  }
+  ctx->cameras[i] = c;
+  *out = c;
+  return 0;
+}
+
+void camera_destroy(EfContext* ctx, EfCamera* c) {
+  ctx->cameras[c->slot - CAMERA_TRACKER0] = nullptr;
+  camera_release(ctx, c);
+}
+
+// ElasticFusion::processFrame (closeLoops = false, reloc = false) at the camera: live side, pose (set, or tracked against the camera's
+// own prediction with its fill-in choice, SO(3) and frameToFrameRGB), weighting, map half at f->time, predict()
+int camera_frame_async(EfContext* ctx, EfCamera* c, const EfCameraFrame* f, const uint8_t* rgb, const uint16_t* depth, bool from_host,
+                       EfCameraResult* out_dev) {
+  const EfCameraConfig& k = c->cfg;
+  const int which = c->slot;
+  OdomDev& od = ctx->odom[which];
+  if (f->has_pose) {  // staged once the previous frame's copy has read the pinned slot (not the whole stream)
+    CU(cudaEventSynchronize(c->pose_sent));
+    memcpy(c->pin_T, f->T_wc, sizeof(double) * 16);
+    CU(cudaMemcpyAsync(c->dev_T, c->pin_T, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaEventRecord(c->pose_sent, ctx->stream));
+  }
+  const LiveBuffers live = {c->rgb, c->rgba, c->depth_raw, c->depth_filtered, c->target.depth_metric, c->target.depth_metric_filtered};
+  RC(track_live_side(ctx, which, live, rgb, depth, true, from_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, k.depth_cutoff,
+                     k.max_depth));
+  const bool tracked = c->has_frame && !f->has_pose;
+  if (!c->has_frame) {
+    // initFirstRGB: this intensity pyramid is the next frame's previous one. The pose is set with itself as the previous pose (the
+    // second k_set_pose), so that the weighting is weight_multiplier.
+    for (int i = 0; i < NUM_PYRS; ++i) std::swap(od.nextImage[i], od.lastNextImage[i]);
+    RC(odom_set_pose_async(ctx, which, c->dev_T));
+    RC(odom_set_pose_async(ctx, which, c->dev_T));
+    RC(odom_finish_async(ctx, which, f->weight_multiplier, false, c->pose));
+  } else if (f->has_pose) {
+    RC(odom_set_pose_async(ctx, which, c->dev_T));
+    RC(odom_finish_async(ctx, which, f->weight_multiplier, false, c->pose));
+  } else {
+    const ModelInputs m = {c->vertex, c->normal, c->fill_vertex, c->fill_normal, c->image, c->fill_image, c->dense_count,
+                           k.frame_to_frame_rgb != 0, c->rgba};
+    RC(track_solve(ctx, which, m, k.rgb_only != 0, k.icp_weight, k.pyramid != 0, k.fast_odom != 0, k.so3 != 0, f->weight_multiplier, c->pose));
+  }
+  // (before predict() recounts the dense samples)
+  EF_LAUNCH(ctx, k_camera_result, 1, 32, 0, (const GNState*)od.gn, (const int*)c->dense_count, k.height, k.width, tracked ? 1 : 0,
+            out_dev ? out_dev : c->result);
+  if (f->fuse && !k.rgb_only) {
+    const MapTarget& t = c->target;
+    RC(map_predict_indices_async(ctx, t, f->time, k.max_depth, k.time_delta));
+    RC(map_fuse_async(ctx, t, f->time, k.max_depth, -1.0f));
+    RC(map_predict_indices_async(ctx, t, f->time, k.max_depth, k.time_delta));
+    RC(map_clean_async(ctx, t, f->time, k.conf_threshold, k.time_delta, k.max_depth));
+  }
+  PredictTarget p = {};
+  p.rows = k.height;
+  p.cols = k.width;
+  p.cx = k.cx;
+  p.cy = k.cy;
+  p.fx = k.fx;
+  p.fy = k.fy;
+  p.pose = c->pose;
+  p.image = c->image;
+  p.vertex = c->vertex;
+  p.normal = c->normal;
+  p.time = c->time;
+  p.dense_count = c->dense_count;
+  p.fill_depth = c->depth_filtered;
+  p.fill_rgb = c->rgb;
+  p.fill_pass_img = k.frame_to_frame_rgb ? 1 : 0;
+  p.fill_image = c->fill_image;
+  p.fill_vertex = c->fill_vertex;
+  p.fill_normal = c->fill_normal;
+  RC(map_predict_target_async(ctx, p, k.max_depth, k.conf_threshold, f->time, f->time, k.time_delta));
+  c->has_frame = true;
+  CHECK_LAST();
+  return 0;
+}
+
+int camera_read(EfContext* ctx, EfCamera* c, EfCameraResult* out, EfSolveTrace* trace, int max_trace, int* n_trace) {
+  int trace_n = 0;
+  CU(cudaMemcpyAsync(out, c->result, sizeof(EfCameraResult), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&trace_n, (const char*)ctx->odom[c->slot].gn + offsetof(GNState, trace_n), sizeof(int), cudaMemcpyDeviceToHost,
+                     ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int n = out->tracked ? (trace_n < max_trace ? trace_n : max_trace) : 0;
+  if (n_trace) *n_trace = n;
+  if (n > 0) {
+    CU(cudaMemcpyAsync(trace, ctx->odom[c->slot].trace, sizeof(EfSolveTrace) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
 }
 
 }  // namespace ef

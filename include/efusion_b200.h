@@ -416,6 +416,78 @@ int ef_track_view(EfContext* ctx, const EfTrackView* view, const uint8_t* rgb, c
 int ef_track_view_device(EfContext* ctx, const EfTrackView* view, const uint8_t* rgb_dev, const uint16_t* depth_dev,
                          EfTrackResult* out_dev);
 
+/* ---- camera: a second RGB-D sensor run frame after frame against the context's map, as ElasticFusion::processFrame
+ *      (Core/ElasticFusion.cpp:270-607, closeLoops = false, reloc = false) runs the context's own camera. A camera belongs to one
+ *      context and has its own tracker (RGBDOdometry of its camera), previous frame, pose, prediction and fill-in; it writes into the
+ *      context's map. One ef_camera_frame runs, at the camera's intrinsics and size:
+ *        1. upload, RGBA, bilateral filter (depth_cutoff) + metric depth, initICP at max_depth and the intensity pyramid (:278-285);
+ *        2. unless has_pose: initICPModel + initRGBModel from the camera's own prediction of its previous call, or from its fill-in
+ *           when that prediction is not dense enough (decided on the device, :302-315; frame_to_frame_rgb takes the fill-in image
+ *           always), the SO(3) pre-alignment against the previous frame's intensity pyramid (so3) and
+ *           getIncrementalTransformation(rgb_only, icp_weight, pyramid, fast_odom, so3);
+ *           with has_pose: the pose is set (processFrame's in_T_wc) and nothing is tracked;
+ *        3. the velocity weighting from the camera's previous pose, times weight_multiplier (:369-383);
+ *        4. fuse and not rgb_only: predictIndices, fuse, predictIndices, clean at `time`, with no graph (:536-585);
+ *        5. predict(): combinedPredict ACTIVE at (time, time, time_delta), then the fill-in from this frame's filtered depth and RGB
+ *           (:621-653) -- the model the camera's next frame tracks against.
+ *      The first frame of a camera must have has_pose (EF_ESTATE otherwise); its intensity pyramid becomes the previous one of the
+ *      next frame (initFirstRGB) and, if it fuses, its weighting is weight_multiplier.
+ *
+ *      A camera writes the surfels and their count, nothing else of the context: not the frame's pose, tick, weighting or pose record,
+ *      any EF_BUF_* buffer, the frame's prediction, fill-in or denseEnough count, the SO(3) or staged frame of the look-ahead, the
+ *      loop-closure state or ef_debug_stage_ms's events. The frame does not re-predict after a camera fused (call ef_predict if it
+ *      should). For a rig: frame A with ef_process_frame*, then the camera with time = ef_get_tick() - 1.
+ *
+ *      fuse = 1 returns EF_ESTATE before the context's first frame and between ef_process_frame_begin and _end (as ef_map_fuse_view);
+ *      fuse = 0 may also run before the first frame, on a map from ef_map_upload. Both may run while the look-ahead holds a staged frame
+ *      and between ef_process_frame_device and ef_finish_frame (stream-ordered). At most EF_MAX_CAMERAS cameras are live per context. */
+#define EF_MAX_CAMERAS 4
+typedef struct EfCamera EfCamera;
+typedef struct {
+  int32_t width, height;          /* 32..4096 */
+  float fx, fy, cx, cy;
+  float depth_cutoff, max_depth;  /* the bilateral filter's maxD (cfg.depth_cutoff); maxDepthProcessed (20), also the map passes' */
+  float conf_threshold;           /* confidenceThreshold of the prediction and the clean (cfg.confidence) */
+  int32_t time_delta;             /* >= 0 (cfg.time_delta) */
+  float icp_weight;               /* >= 0 (10; >= 100: ICP only) */
+  int32_t rgb_only, pyramid, fast_odom, so3, frame_to_frame_rgb;  /* the frame's setters (0, 1, cfg.fast_odom, cfg.so3, ...) */
+} EfCameraConfig;
+typedef struct {
+  int32_t time;                   /* >= 0: the tick this frame's surfels are stamped with and its prediction is made at */
+  float weight_multiplier;        /* finite, >= 0 */
+  int32_t has_pose;               /* set the pose T_wc instead of tracking (processFrame's in_T_wc) */
+  double T_wc[16];                /* row-major camera-to-world, read when has_pose */
+  int32_t fuse;                   /* 0: track and predict only (localise in a fixed map) */
+} EfCameraFrame;
+typedef struct {
+  double T_wc[16];                /* the camera's pose after the frame */
+  EfOdomStats stats;              /* its tracker's, as ef_odom_stats reports them */
+  double covariance[36];          /* lastA^-1, as ef_odom_covariance */
+  int32_t tracked;                /* 0 when the pose came from has_pose */
+  int32_t dense_enough;           /* denseEnough of the prediction this frame tracked against (0: the fill-in was used) */
+  float weighting;                /* the fusion weighting (ElasticFusion.cpp:369-383) */
+} EfCameraResult;
+/* EF_EINVAL for a NULL argument or a bad field (a size outside 32..4096, a zero or non-finite fx / fy, a non-finite cx / cy,
+ * depth_cutoff or max_depth not finite and > 0, a non-finite conf_threshold, a negative time_delta, a non-finite or negative
+ * icp_weight); EF_ESTATE when EF_MAX_CAMERAS cameras are live; EF_ENOMEM when its buffers cannot be allocated (the context stays
+ * usable). Memory: see INTEGRATION.md. Synchronises. */
+int ef_camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out);
+/* frees the camera (ef_destroy frees those still live); EF_EINVAL for a camera of another context. Synchronises. */
+int ef_camera_destroy(EfContext* ctx, EfCamera* cam);
+/* HOST inputs RGB8 (W*H*3 B) and uint16 millimetres (W*H); synchronises. trace (HOST, may be NULL when max_trace = 0) receives one
+ * record per Gauss-Newton iteration of a tracked frame. EF_EINVAL for a NULL argument, a camera of another context, a negative time,
+ * a bad weight_multiplier, a non-finite pose entry with has_pose, or a negative max_trace. */
+int ef_camera_frame(EfContext* ctx, EfCamera* cam, const EfCameraFrame* frame, const uint8_t* rgb, const uint16_t* depth,
+                    EfCameraResult* out, EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace);
+/* same from DEVICE inputs into a DEVICE result, asynchronous on ef_stream(); EF_EINVAL also for a depth pointer not aligned to 2
+ * bytes or out_dev not aligned to 8 */
+int ef_camera_frame_device(EfContext* ctx, EfCamera* cam, const EfCameraFrame* frame, const uint8_t* rgb_dev, const uint16_t* depth_dev,
+                           EfCameraResult* out_dev);
+/* device pointer + byte size of a buffer of the camera, at its size: EF_BUF_RGB, RGBA, DEPTH_* (its inputs), IMAGE, VERTEX, NORMAL,
+ * TIME (its prediction), FILL_* (its fill-in) and the tracker ids 40..53 without the 100*which (its pyramids, `level`). Any other id:
+ * EF_EINVAL. */
+int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32_t level, void** dev_ptr, size_t* bytes);
+
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
   /* input / preprocess textures (ElasticFusion::textures, GPUTexture.cpp:22-27) */
