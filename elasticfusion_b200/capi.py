@@ -142,7 +142,7 @@ class EfCameraConfig(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
                 ("depth_cutoff", C.c_float), ("max_depth", C.c_float), ("conf_threshold", C.c_float), ("time_delta", C.c_int32),
                 ("icp_weight", C.c_float), ("rgb_only", C.c_int32), ("pyramid", C.c_int32), ("fast_odom", C.c_int32), ("so3", C.c_int32),
-                ("frame_to_frame_rgb", C.c_int32)]
+                ("frame_to_frame_rgb", C.c_int32), ("close_loops", C.c_int32)]
 
 
 class EfCameraFrame(C.Structure):
@@ -159,9 +159,10 @@ MAX_CAMERAS = 4  # EF_MAX_CAMERAS
 
 
 def camera_config(w, h, fx, fy, cx, cy, depth_cutoff=3.0, max_depth=20.0, conf_threshold=10.0, time_delta=200, icp_weight=10.0,
-                  rgb_only=False, pyramid=True, fast_odom=False, so3=True, frame_to_frame_rgb=False) -> EfCameraConfig:
+                  rgb_only=False, pyramid=True, fast_odom=False, so3=True, frame_to_frame_rgb=False, close_loops=False) -> EfCameraConfig:
     """EfCameraConfig of a w x h pinhole camera. The defaults are the frame's (ef_default_config and the ElasticFusion constructor):
-    depth_cutoff 3 m, maxDepthProcessed 20 m, confidence 10, time_delta 200, icp_weight 10, pyramid and SO(3) on."""
+    depth_cutoff 3 m, maxDepthProcessed 20 m, confidence 10, time_delta 200, icp_weight 10, pyramid and SO(3) on. close_loops: its
+    frames close local loops on the context's graph (a context with close_loops = 2)."""
     c = EfCameraConfig()
     c.width, c.height = int(w), int(h)
     c.fx, c.fy, c.cx, c.cy = float(fx), float(fy), float(cx), float(cy)
@@ -169,6 +170,7 @@ def camera_config(w, h, fx, fy, cx, cy, depth_cutoff=3.0, max_depth=20.0, conf_t
     c.time_delta, c.icp_weight = int(time_delta), float(icp_weight)
     c.rgb_only, c.pyramid, c.fast_odom = int(bool(rgb_only)), int(bool(pyramid)), int(bool(fast_odom))
     c.so3, c.frame_to_frame_rgb = int(bool(so3)), int(bool(frame_to_frame_rgb))
+    c.close_loops = int(bool(close_loops))
     return c
 
 
@@ -180,6 +182,17 @@ def camera_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfCameraF
         f.has_pose = 1
         f.T_wc[:] = np.asarray(T_wc, np.float64).reshape(16).tolist()
     return f
+
+
+def _local_deform(call):
+    """(info dict, graph (n, 4) float32) of ef_local_deform_result or ef_camera_deform_result, called as call(out, nodes, n_out)"""
+    res = EfLocalDeform()
+    nodes = np.zeros((1023, 4), np.float32)
+    n = C.c_int32()
+    _chk(call(C.byref(res), nodes, C.byref(n)))
+    info = dict(solved=bool(res.solved), applied=bool(res.applied), result={k: getattr(res.result, k) for k, _ in EfDeformResult._fields_},
+                deforms=res.deforms, last_deform_time=res.last_deform_time, n_nodes=res.n_nodes)
+    return info, nodes[:n.value].copy()
 
 
 def unpack_camera_result(res):
@@ -410,13 +423,7 @@ class Context:
     def local_deform_result(self):
         """close_loops = 2: (info dict, graph (n, 4) float32: x y z time per node) of the last frame's in-frame loop closure.
         info: solved, applied, result (EfDeformResult fields, all zero unless solved), deforms, last_deform_time, n_nodes."""
-        res = EfLocalDeform()
-        nodes = np.zeros((1023, 4), np.float32)
-        n = C.c_int32()
-        _chk(lib().ef_local_deform_result(self.h_ctx, C.byref(res), _p(nodes), len(nodes), C.byref(n)))
-        info = dict(solved=bool(res.solved), applied=bool(res.applied), result={k: getattr(res.result, k) for k, _ in EfDeformResult._fields_},
-                    deforms=res.deforms, last_deform_time=res.last_deform_time, n_nodes=res.n_nodes)
-        return info, nodes[:n.value].copy()
+        return _local_deform(lambda res, nodes, n: lib().ef_local_deform_result(self.h_ctx, res, _p(nodes), len(nodes), n))
 
     def predict(self):
         _chk(lib().ef_predict(self.h_ctx))
@@ -696,6 +703,11 @@ class Camera:
         f = camera_frame(time, weight_multiplier, T_wc, fuse)
         _chk(lib().ef_camera_frame_device(self.ctx.h_ctx, self.h_cam, C.byref(f), C.c_void_p(rgb_ptr or None), C.c_void_p(depth_ptr or None),
                                           C.c_void_p(result_ptr or None)))
+
+    def deform_result(self):
+        """close_loops: (info dict, graph) of the camera's last frame, as Context.local_deform_result returns them (solved, applied and
+        result are the camera's; deforms, last_deform_time and the graph the context's)."""
+        return _local_deform(lambda res, nodes, n: lib().ef_camera_deform_result(self.ctx.h_ctx, self.h_cam, res, _p(nodes), len(nodes), n))
 
     def buffer_ptr(self, name, level=0):
         ptr, nbytes = C.c_void_p(), C.c_size_t()

@@ -17,10 +17,12 @@ constexpr int MAX_RED_BLOCKS = 1184; // 8 resident 256-thread CTAs per SM on up 
 constexpr int PARTIAL_STRIDE = 64;   // floats per CTA partial: [0,29) geometric system, [32,61) photometric system
 constexpr int MAX_TRACE = 48;
 // tracker slots of EfContext::odom: 0 frameToModel, 1 modelToModel (both sized for the context's camera), the tracker of
-// ef_track_view*, whose buffers are sized for the largest view so far, and one per live EfCamera, sized for its camera
+// ef_track_view*, whose buffers are sized for the largest view so far, one per live EfCamera, sized for its camera, and the
+// modelToModel tracker of each camera that closes loops (CAMERA_LOOP_TRACKER0 + the camera's index)
 constexpr int VIEW_TRACKER = 2;
 constexpr int CAMERA_TRACKER0 = 3;
-constexpr int NUM_TRACKERS = CAMERA_TRACKER0 + EF_MAX_CAMERAS;
+constexpr int CAMERA_LOOP_TRACKER0 = CAMERA_TRACKER0 + EF_MAX_CAMERAS;
+constexpr int NUM_TRACKERS = CAMERA_LOOP_TRACKER0 + EF_MAX_CAMERAS;
 constexpr int DENSE_FACTOR = 20;  // ElasticFusion::denseEnough decimates the predicted image by 20 (ElasticFusion.cpp:258)
 
 // ElasticFusion::denseEnough (ElasticFusion.cpp:256-268) from the number of lit samples of the decimated image
@@ -157,7 +159,7 @@ struct OdomDev {
 constexpr int MAX_GRAPH_NODES = 1024;  // GlobalModel::MAX_NODES = 16384 / 16 (GlobalModel.cpp:25-26)
 
 // device-resident result of the local loop closure front half (ElasticFusion.cpp:447-505); the constraint pairs themselves
-// live in MapDev::loop_src / loop_dst / loop_times, sized from the frame
+// live in MapDev::loop_src / loop_dst / loop_times, sized from the frame (a closing camera's in LoopBuffers of its own)
 struct LoopDev {
   int ran, accepted, n_constraints;
   float lastICPError, lastICPCount;
@@ -275,8 +277,8 @@ struct PinStaging {
   double T_wc[16];       // frame_begin_device: the caller's pose for a frame that is not tracked
   double finish_T_wc[16];  // ef_finish_frame: pose and surfel count read back
   int finish_count;
-  int loop_record[3];              // close_loops = 2, mid-frame: LoopDev::accepted, LoopDev::n_constraints, MapDev::graph_n
-  EfDeformResult deform_result;    // close_loops = 2: the frame's deformation solve
+  int loop_record[3];              // loop_solve_apply: LoopDev::accepted, LoopDev::n_constraints, MapDev::graph_n
+  EfDeformResult deform_result;    // loop_solve_apply: the deformation solve of the frame or a closing camera
   double view_pose[16];  // stage_view_pose: T_wc of a model or fuse view (rewritten after EfContext::view_pose_sent, not a sync)
   float view_weighting;  // stage_view_pose: fusion weighting of a fuse view (same guard)
 };
@@ -312,7 +314,7 @@ struct MapTarget {
   float cx, cy, fx, fy;
   const uint8_t* rgb;  // W*H*3
   float *depth_metric, *depth_metric_filtered;
-  const float* synth_depth;  // read by the clean's time-stamp refresh under a deformation graph (the frame's only)
+  const float* synth_depth;  // read by the clean's time-stamp refresh under a deformation graph (the frame's or a closing camera's)
   MapPose* pose;
   float* weighting;          // device: fuse's confidence weighting
   // index map: tagged keys (key_texels of them, all re-armed when the tags run out) and the four textures
@@ -341,12 +343,50 @@ struct PredictTarget {
   uchar4* image;
   float4 *vertex, *normal;
   uint16_t* time;
+  float* depth;                // given: the synthesised depth alone (synthesizeDepth), and none of the outputs above
   int* dense_count;
   const uint16_t* fill_depth;  // W*H filtered millimetres
   const uint8_t* fill_rgb;     // W*H*3
   int fill_pass_img;           // frameToFrameRGB: the fill-in image is the live RGB everywhere
   uchar4* fill_image;
   float4 *fill_vertex, *fill_normal;
+};
+
+// What the local loop closure of one camera works on (ElasticFusion.cpp:447-534): the frame's (tracker 0 and modelToModel tracker 1,
+// MapDev's loop buffers, Textures' predictions) or a closing camera's (its tracker, its loop tracker and LoopBuffers)
+struct LoopSide {
+  int curr, est;             // tracker slots: the camera's (T_wc_curr) and its modelToModel tracker
+  int rows, cols;
+  float max_depth;
+  bool pyramid, fast_odom;
+  const float4 *vertex, *normal;  // the ACTIVE prediction of the mid-frame predict()
+  const uchar4* image;
+  const float4 *old_vertex, *old_normal;  // the INACTIVE prediction
+  const uchar4* old_image;
+  const uint16_t* old_time;
+  LoopDev* loop;
+  double *src, *dst;
+  int* times;
+  int capacity;
+};
+
+// A closing camera's buffers of the local loop closure, at its size (ef_camera_* with close_loops = 1)
+struct LoopBuffers {
+  uchar4* old_image;  // INACTIVE prediction at (0, time - time_delta, time_delta)
+  float4 *old_vertex, *old_normal;
+  uint16_t* old_time;
+  float* synth_depth;  // the deformed clean's depth-only prediction
+  LoopDev* loop;
+  double *src, *dst;
+  int* times;
+  int capacity;
+  ScanTiles scan;      // look-back tile states of the loop tracker's candidate compaction
+};
+
+// The outcome of the last local closure of one side (the frame, or a closing camera)
+struct DeformOutcome {
+  bool solved, applied;
+  EfDeformResult result;
 };
 
 }  // namespace ef
@@ -388,10 +428,10 @@ struct EfContext {
   float confidence, depth_cutoff, max_depth_processed;
   int host_count;  // last count read back
   bool frame_open; // ef_process_frame_begin has run, ef_process_frame_end has not
-  // close_loops = 2: Deformation's bookkeeping (ElasticFusion::deforms, Deformation::lastDeformTime) and the last frame's outcome
+  // close_loops = 2: Deformation's bookkeeping (ElasticFusion::deforms, Deformation::lastDeformTime), shared with the closing cameras,
+  // and the last frame's outcome
   int deforms, last_deform_time;
-  bool deform_solved, deform_applied;
-  EfDeformResult deform_result;
+  ef::DeformOutcome deform_out;
 
   // pinned staging
   uint8_t* pin_rgb;
@@ -429,6 +469,9 @@ struct EfCamera {
   ef::MapTarget target;    // its map-write side (pose record and tracker weighting set)
   void* target_state;      // map_camera_target's
   EfCameraResult* result;  // device: the result of its last frame (the host call reads it back)
+  ef::LoopBuffers loop;    // close_loops = 1: its local loop closure (tracker slot loop_slot)
+  int loop_slot;
+  ef::DeformOutcome deform_out;  // close_loops = 1: its last frame's closure
   double* pin_T;           // pinned staging of a frame's has_pose T_wc, rewritten after pose_sent
   double* dev_T;
   cudaEvent_t pose_sent;
@@ -518,6 +561,12 @@ namespace ef {
 // `arena`; synchronises ctx->stream
 int alloc_odom(EfContext* ctx, Arena& arena, int which, int width, int height, float fx, float fy, float cx, float cy);
 
+// ef_api.cu: the local loop closure of one side. loop_front_half: the front half after its INACTIVE prediction (ElasticFusion.cpp:
+// 457-505); loop_solve_apply: the read-back, solve and hand-over (:505-526) at `time`, the pose going to tracker s.curr and pose_record;
+// *n_nodes: the graph the clean applies (0: none)
+int loop_front_half(EfContext* ctx, const LoopSide& s);
+int loop_solve_apply(EfContext* ctx, const LoopSide& s, int time, MapPose* pose_record, DeformOutcome* out, int* n_nodes);
+
 // ef_track.cu: the tracker's input pyramids
 int odom_init_icp_depth(EfContext* ctx, int which, const uint16_t* depth_dev, float cutoff);
 int odom_init_icp_pred(EfContext* ctx, int which, const float* vtx4, const float* nrm4);
@@ -602,8 +651,11 @@ int map_predict_view_async(EfContext* ctx, const EfModelView* view, uint8_t* ima
 // the same at t.pose (device), writing t's outputs, dense count and fill-in
 int map_predict_target_async(EfContext* ctx, const PredictTarget& t, float max_depth, float conf_threshold, int time, int max_time, int time_delta);
 int map_dense_enough_async(EfContext* ctx);
-int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh);
-int map_loop_reset_async(EfContext* ctx);
+// the acceptance test and the constraints of side s's front half, with the context's thresholds
+int map_loop_constraints_async(EfContext* ctx, const LoopSide& s);
+int map_loop_reset_async(EfContext* ctx, LoopDev* loop);
+// the map kernels' pose record `mp` from a device T_wc
+int map_pose_record_async(EfContext* ctx, MapPose* mp, const double* T_dev);
 int odom_copy_pose_async(EfContext* ctx, int dst, int src);
 int map_download(EfContext* ctx, const float4* a, const float4* b, const float4* c, int n, float* out);
 int map_upload(EfContext* ctx, const float* in, int n);

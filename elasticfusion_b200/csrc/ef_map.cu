@@ -1587,7 +1587,11 @@ int map_update_pose_async(EfContext* ctx, const double* T_host) {
     CU(cudaMemcpyAsync(ctx->dev_small->map_pose, ctx->pin_small->map_pose, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
     src = ctx->dev_small->map_pose;
   }
-  EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, ctx->map.pose, src);
+  return map_pose_record_async(ctx, ctx->map.pose, src);
+}
+
+int map_pose_record_async(EfContext* ctx, MapPose* mp, const double* T_dev) {
+  EF_LAUNCH(ctx, k_update_pose, 1, 32, 0, mp, T_dev);
   CHECK_LAST();
   return 0;
 }
@@ -1837,16 +1841,17 @@ static int stage_view_pose(EfContext* ctx, const double* T_wc, float weighting) 
   return 0;
 }
 
-// the raycast above at a camera of its own and the pose record `pose`, on the off-frame z-buffer; f: its dense count and fill-in
+// the raycast above at a camera of its own and the pose record `pose`, on the off-frame z-buffer; f: its dense count and fill-in;
+// depth given: the synthesised depth alone
 static int predict_offframe(EfContext* ctx, const RayArgs& a, const MapPose* pose, uchar4* image, float4* vertex, float4* normal, uint16_t* time,
-                            const FillOut& f) {
+                            const FillOut& f, float* depth = nullptr) {
   MapDev& m = ctx->map;
   const size_t n = (size_t)a.rows * a.cols;
   unsigned long long* zbuf = nullptr;
   RC(offframe_zbuf(ctx, n, &zbuf));
   EF_LAUNCH(ctx, k_splat_scatter, ctx->num_sms * 4, SPLAT_THREADS, 0, a, pose, m.pos_conf, m.color_time, m.norm_rad, m.count, zbuf, f.dense_count);
   EF_LAUNCH(ctx, k_splat_resolve, wave_blocks(ctx, n), 256, 0, a, pose, m.pos_conf, m.color_time, m.norm_rad, zbuf, image, vertex, normal, time,
-            (float*)nullptr, f);
+            depth, f);
   CHECK_LAST();
   return 0;
 }
@@ -1887,7 +1892,7 @@ int map_predict_target_async(EfContext* ctx, const PredictTarget& t, float max_d
     f.image = t.fill_image;
   }
   return predict_offframe(ctx, ray_args(t.rows, t.cols, Cam{t.cx, t.cy, t.fx, t.fy}, max_depth, conf_threshold, time, max_time, time_delta),
-                          t.pose, t.image, t.vertex, t.normal, t.time, f);
+                          t.pose, t.image, t.vertex, t.normal, t.time, f, t.depth);
 }
 
 // ---- fuse view (ef_map_fuse_view*): its own inputs, index map and scratch, in one allocation grown to the largest view ----
@@ -2263,16 +2268,15 @@ __global__ void k_copy_pose(GNState* dst, const GNState* src) {
   if (blockIdx.x == 0 && threadIdx.x < 16) dst->T_wc[threadIdx.x] = src->T_wc[threadIdx.x];
 }
 
-int map_loop_constraints_async(EfContext* ctx, int count_thresh, float err_thresh, float cov_thresh) {
-  MapDev& m = ctx->map;
-  EF_LAUNCH(ctx, k_loop_constraints, 1, 256, 0, (const GNState*)ctx->odom[0].gn, (const GNState*)ctx->odom[1].gn, (const float4*)ctx->tex.vertex,
-            (const uint16_t*)ctx->tex.old_time, m.rows, m.cols, ctx->max_depth_processed, count_thresh, err_thresh, cov_thresh, m.loop,
-            m.loop_src, m.loop_dst, m.loop_times, m.loop_capacity);
+int map_loop_constraints_async(EfContext* ctx, const LoopSide& s) {
+  const EfConfig& c = ctx->cfg;
+  EF_LAUNCH(ctx, k_loop_constraints, 1, 256, 0, (const GNState*)ctx->odom[s.curr].gn, (const GNState*)ctx->odom[s.est].gn, s.vertex, s.old_time,
+            s.rows, s.cols, s.max_depth, c.count_thresh, c.err_thresh, c.cov_thresh, s.loop, s.src, s.dst, s.times, s.capacity);
   CHECK_LAST();
   return 0;
 }
-int map_loop_reset_async(EfContext* ctx) {
-  EF_LAUNCH(ctx, k_loop_reset, 1, 32, 0, ctx->map.loop);
+int map_loop_reset_async(EfContext* ctx, LoopDev* loop) {
+  EF_LAUNCH(ctx, k_loop_reset, 1, 32, 0, loop);
   CHECK_LAST();
   return 0;
 }

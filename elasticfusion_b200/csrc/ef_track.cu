@@ -868,6 +868,22 @@ static int camera_alloc(EfContext* ctx, EfCamera& c) {
   RC(map_camera_target(ctx, c.arena, k.height, k.width, k.fx, k.fy, k.cx, k.cy, &c.target_state, &c.target, &c.rgb, &c.depth_raw));
   c.target.pose = c.pose;
   c.target.weighting = &ctx->odom[c.slot].gn->weighting;
+  if (k.close_loops) {  // its local loop closure: a modelToModel tracker, the INACTIVE prediction, the synthesised depth, the constraints
+    LoopBuffers& L = c.loop;
+    RC(alloc_odom(ctx, c.arena, c.loop_slot, k.width, k.height, k.fx, k.fy, k.cx, k.cy));
+    RC(alloc_cand_tiles(ctx, c.arena, c.loop_slot, L.scan));
+    CU(arena_alloc(ctx, c.arena, &L.old_image, px, 0));
+    CU(arena_alloc(ctx, c.arena, &L.old_vertex, px, 0));
+    CU(arena_alloc(ctx, c.arena, &L.old_normal, px, 0));
+    CU(arena_alloc(ctx, c.arena, &L.old_time, px, 0));
+    CU(arena_alloc(ctx, c.arena, &L.synth_depth, px, 0));
+    CU(arena_alloc(ctx, c.arena, &L.loop, 1, 0));
+    L.capacity = loop_constraint_capacity(k.width, k.height);
+    CU(arena_alloc(ctx, c.arena, &L.src, 3 * (size_t)L.capacity, 0));
+    CU(arena_alloc(ctx, c.arena, &L.dst, 3 * (size_t)L.capacity, 0));
+    CU(arena_alloc(ctx, c.arena, &L.times, (size_t)L.capacity, 0));
+    c.target.synth_depth = L.synth_depth;
+  }
   unsigned long long* zbuf = nullptr;
   RC(offframe_zbuf(ctx, px, &zbuf));  // grown here, so that a frame never allocates
   CU(cudaMallocHost((void**)&c.pin_T, sizeof(double) * 16));
@@ -884,8 +900,10 @@ static void camera_release(EfContext* ctx, EfCamera* c) {
   if (c->target_state) map_camera_target_free(c->target_state);
   if (c->pin_T) cudaFreeHost(c->pin_T);
   if (c->pose_sent) cudaEventDestroy(c->pose_sent);
-  memset(&ctx->odom[c->slot], 0, sizeof(OdomDev));
-  ctx->odom_tiles[c->slot] = nullptr;
+  for (int w : {c->slot, c->loop_slot}) {
+    memset(&ctx->odom[w], 0, sizeof(OdomDev));
+    ctx->odom_tiles[w] = nullptr;
+  }
   delete c;
 }
 
@@ -896,6 +914,7 @@ int camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out) {
   EfCamera* c = new (std::nothrow) EfCamera();
   if (!c) return EF_ENOMEM;
   c->slot = CAMERA_TRACKER0 + i;
+  c->loop_slot = CAMERA_LOOP_TRACKER0 + i;
   c->cfg = *cfg;
   if (int rc = camera_alloc(ctx, *c)) {
     camera_release(ctx, c);
@@ -913,8 +932,75 @@ void camera_destroy(EfContext* ctx, EfCamera* c) {
   camera_release(ctx, c);
 }
 
-// ElasticFusion::processFrame (closeLoops = false, reloc = false) at the camera: live side, pose (set, or tracked against the camera's
-// own prediction with its fill-in choice, SO(3) and frameToFrameRGB), weighting, map half at f->time, predict()
+// combinedPredict at the camera's pose record, size and intrinsics, into nothing yet
+static PredictTarget camera_predict_target(const EfCamera* c) {
+  const EfCameraConfig& k = c->cfg;
+  PredictTarget p = {};
+  p.rows = k.height;
+  p.cols = k.width;
+  p.cx = k.cx;
+  p.cy = k.cy;
+  p.fx = k.fx;
+  p.fy = k.fy;
+  p.pose = c->pose;
+  return p;
+}
+
+// a closing camera's side of the local loop closure: its tracker, its loop tracker, its prediction and LoopBuffers
+static LoopSide camera_loop_side(const EfCamera* c) {
+  const EfCameraConfig& k = c->cfg;
+  const LoopBuffers& L = c->loop;
+  LoopSide s = {};
+  s.curr = c->slot;
+  s.est = c->loop_slot;
+  s.rows = k.height;
+  s.cols = k.width;
+  s.max_depth = k.max_depth;
+  s.pyramid = k.pyramid != 0;
+  s.fast_odom = k.fast_odom != 0;
+  s.vertex = c->vertex;
+  s.normal = c->normal;
+  s.image = c->image;
+  s.old_vertex = L.old_vertex;
+  s.old_normal = L.old_normal;
+  s.old_image = L.old_image;
+  s.old_time = L.old_time;
+  s.loop = L.loop;
+  s.src = L.src;
+  s.dst = L.dst;
+  s.times = L.times;
+  s.capacity = L.capacity;
+  return s;
+}
+
+// close_loops = 1, on a fused frame after the first: the mid-frame predict() ACTIVE at (time, time, time_delta) (ElasticFusion.cpp:387;
+// its fill-in and dense count are left out: only the front half reads this prediction, and the end-of-frame predict() rewrites all of
+// it), the INACTIVE prediction at (0, time - time_delta, time_delta), the front half and the closure at `time`. The result's pose
+// becomes the closed one. *n_nodes: the graph the camera's clean applies.
+static int camera_close_loop(EfContext* ctx, EfCamera* c, int time, EfCameraResult* result, int* n_nodes) {
+  const EfCameraConfig& k = c->cfg;
+  PredictTarget p = camera_predict_target(c);
+  p.image = c->image;
+  p.vertex = c->vertex;
+  p.normal = c->normal;
+  p.time = c->time;
+  RC(map_predict_target_async(ctx, p, k.max_depth, k.conf_threshold, time, time, k.time_delta));
+  p.image = c->loop.old_image;
+  p.vertex = c->loop.old_vertex;
+  p.normal = c->loop.old_normal;
+  p.time = c->loop.old_time;
+  RC(map_predict_target_async(ctx, p, k.max_depth, k.conf_threshold, 0, time - k.time_delta, k.time_delta));
+  const LoopSide s = camera_loop_side(c);
+  RC(loop_front_half(ctx, s));
+  RC(loop_solve_apply(ctx, s, time, c->pose, &c->deform_out, n_nodes));
+  if (c->deform_out.applied)
+    CU(cudaMemcpyAsync(result->T_wc, ctx->odom[c->slot].gn->T_wc, sizeof(double) * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+  return 0;
+}
+
+// ElasticFusion::processFrame (reloc = false) at the camera: live side, pose (set, or tracked against the camera's own prediction with
+// its fill-in choice, SO(3) and frameToFrameRGB), weighting, with close_loops the local loop closure (camera_close_loop), map half at
+// f->time, predict() and, with close_loops, the graph sampled from the map the call leaves (:593)
 int camera_frame_async(EfContext* ctx, EfCamera* c, const EfCameraFrame* f, const uint8_t* rgb, const uint16_t* depth, bool from_host,
                        EfCameraResult* out_dev) {
   const EfCameraConfig& k = c->cfg;
@@ -930,6 +1016,8 @@ int camera_frame_async(EfContext* ctx, EfCamera* c, const EfCameraFrame* f, cons
   RC(track_live_side(ctx, which, live, rgb, depth, true, from_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, k.depth_cutoff,
                      k.max_depth));
   const bool tracked = c->has_frame && !f->has_pose;
+  const bool map_half = f->fuse && !k.rgb_only;
+  const bool front_half = k.close_loops && map_half && c->has_frame;
   if (!c->has_frame) {
     // initFirstRGB: this intensity pyramid is the next frame's previous one. The pose is set with itself as the previous pose (the
     // second k_set_pose), so that the weighting is weight_multiplier.
@@ -946,23 +1034,24 @@ int camera_frame_async(EfContext* ctx, EfCamera* c, const EfCameraFrame* f, cons
     RC(track_solve(ctx, which, m, k.rgb_only != 0, k.icp_weight, k.pyramid != 0, k.fast_odom != 0, k.so3 != 0, f->weight_multiplier, c->pose));
   }
   // (before predict() recounts the dense samples)
-  EF_LAUNCH(ctx, k_camera_result, 1, 32, 0, (const GNState*)od.gn, (const int*)c->dense_count, k.height, k.width, tracked ? 1 : 0,
-            out_dev ? out_dev : c->result);
-  if (f->fuse && !k.rgb_only) {
+  EfCameraResult* result = out_dev ? out_dev : c->result;
+  EF_LAUNCH(ctx, k_camera_result, 1, 32, 0, (const GNState*)od.gn, (const int*)c->dense_count, k.height, k.width, tracked ? 1 : 0, result);
+  memset(&c->deform_out, 0, sizeof(c->deform_out));
+  int n_nodes = 0;
+  if (front_half) RC(camera_close_loop(ctx, c, f->time, result, &n_nodes));
+  if (map_half) {
     const MapTarget& t = c->target;
     RC(map_predict_indices_async(ctx, t, f->time, k.max_depth, k.time_delta));
     RC(map_fuse_async(ctx, t, f->time, k.max_depth, -1.0f));
     RC(map_predict_indices_async(ctx, t, f->time, k.max_depth, k.time_delta));
-    RC(map_clean_async(ctx, t, f->time, k.conf_threshold, k.time_delta, k.max_depth));
+    if (n_nodes > 0) {  // ElasticFusion.cpp:559-569: the time-stamp refresh of deformed surfels reads this depth
+      PredictTarget d = camera_predict_target(c);
+      d.depth = c->loop.synth_depth;
+      RC(map_predict_target_async(ctx, d, k.max_depth, k.conf_threshold, f->time, f->time - k.time_delta, 65535));
+    }
+    RC(map_clean_async(ctx, t, f->time, k.conf_threshold, k.time_delta, k.max_depth, n_nodes));
   }
-  PredictTarget p = {};
-  p.rows = k.height;
-  p.cols = k.width;
-  p.cx = k.cx;
-  p.cy = k.cy;
-  p.fx = k.fx;
-  p.fy = k.fy;
-  p.pose = c->pose;
+  PredictTarget p = camera_predict_target(c);
   p.image = c->image;
   p.vertex = c->vertex;
   p.normal = c->normal;
@@ -975,6 +1064,7 @@ int camera_frame_async(EfContext* ctx, EfCamera* c, const EfCameraFrame* f, cons
   p.fill_vertex = c->fill_vertex;
   p.fill_normal = c->fill_normal;
   RC(map_predict_target_async(ctx, p, k.max_depth, k.conf_threshold, f->time, f->time, k.time_delta));
+  if (k.close_loops) RC(map_sample_graph_async(ctx));
   c->has_frame = true;
   CHECK_LAST();
   return 0;

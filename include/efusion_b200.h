@@ -157,8 +157,9 @@ typedef struct {
   int32_t solved;            /* the last frame ran the solve */
   int32_t applied;           /* ... and applied its graph and pose */
   EfDeformResult result;     /* that solve's result; all zero when !solved */
-  int32_t deforms;           /* closures applied since ef_create (ElasticFusion::getDeforms) */
-  int32_t last_deform_time;  /* tick of the last applied closure (Deformation::lastDeformTime); 0 before the first */
+  int32_t deforms;           /* closures applied since ef_create (ElasticFusion::getDeforms), a closing camera's included */
+  int32_t last_deform_time;  /* tick (a closing camera's: time) of the last applied closure (Deformation::lastDeformTime); 0 before
+                                the first */
   int32_t n_nodes;           /* nodes of the current graph (0: none sampled yet) */
 } EfLocalDeform;
 /* nodes4 (HOST, may be NULL when max_nodes = 0): the current graph, x y z and time per node (Deformation::rawSampledNodes_w);
@@ -438,6 +439,22 @@ int ef_track_view_device(EfContext* ctx, const EfTrackView* view, const uint8_t*
  *      loop-closure state or ef_debug_stage_ms's events. The frame does not re-predict after a camera fused (call ef_predict if it
  *      should). For a rig: frame A with ef_process_frame*, then the camera with time = ef_get_tick() - 1.
  *
+ *      With close_loops = 1 (a context with cfg.close_loops = 2 only), a camera's frames close local loops as the frame does in that
+ *      mode (Core/ElasticFusion.cpp:387, 447-534, 559-569 and 593), at the camera's intrinsics, size and `time` in place of the tick:
+ *        - on a fused, not rgb_only frame after the camera's first (has_pose frames too): after step 3, predict() ACTIVE at (time, time,
+ *          time_delta), the INACTIVE prediction at (0, time - time_delta, time_delta), model-to-model tracking in a second tracker of the
+ *          camera, the acceptance test with the context's count_thresh / err_thresh / cov_thresh and the constraints on its
+ *          (W/20) x (H/20) grid; on an accepted front half with a graph and a constraint, the solve of ef_local_deform_result
+ *          (pin = (deforms == 0), source time `time`) and, unless it stops with code 6, its pose becomes T_wc_est and step 4's clean
+ *          deforms the map with the nodes (its time-stamp refresh reads a depth-only prediction at (time, time - time_delta, 65535));
+ *          then deforms += 1 and last_deform_time = time;
+ *        - at the end of every call, the graph is sampled from the map (fuse = 0 and first calls too).
+ *      EfCameraResult.T_wc is then the pose after the closure; the weighting is the one computed before it. Besides the surfels and
+ *      their count, a closing camera writes the context's graph, deforms and last_deform_time (none of the frame's other loop-closure
+ *      results: see ef_camera_deform_result). ef_camera_frame_device then waits for the host once for the front half's record and, on a
+ *      frame that solves, once more for the solve (as ef_process_frame_device does with cfg.close_loops = 2). The side that did not
+ *      deform the map keeps tracking against the prediction it made before the closure.
+ *
  *      fuse = 1 returns EF_ESTATE before the context's first frame and between ef_process_frame_begin and _end (as ef_map_fuse_view);
  *      fuse = 0 may also run before the first frame, on a map from ef_map_upload. Both may run while the look-ahead holds a staged frame
  *      and between ef_process_frame_device and ef_finish_frame (stream-ordered). At most EF_MAX_CAMERAS cameras are live per context. */
@@ -451,6 +468,7 @@ typedef struct {
   int32_t time_delta;             /* >= 0 (cfg.time_delta) */
   float icp_weight;               /* >= 0 (10; >= 100: ICP only) */
   int32_t rgb_only, pyramid, fast_odom, so3, frame_to_frame_rgb;  /* the frame's setters (0, 1, cfg.fast_odom, cfg.so3, ...) */
+  int32_t close_loops;            /* 0: open loop. 1: its frames close local loops on the context's graph (cfg.close_loops = 2 only) */
 } EfCameraConfig;
 typedef struct {
   int32_t time;                   /* >= 0: the tick this frame's surfels are stamped with and its prediction is made at */
@@ -469,7 +487,7 @@ typedef struct {
 } EfCameraResult;
 /* EF_EINVAL for a NULL argument or a bad field (a size outside 32..4096, a zero or non-finite fx / fy, a non-finite cx / cy,
  * depth_cutoff or max_depth not finite and > 0, a non-finite conf_threshold, a negative time_delta, a non-finite or negative
- * icp_weight); EF_ESTATE when EF_MAX_CAMERAS cameras are live; EF_ENOMEM when its buffers cannot be allocated (the context stays
+ * icp_weight, close_loops other than 0 or 1, or 1 on a context whose cfg.close_loops is not 2); EF_ESTATE when EF_MAX_CAMERAS cameras are live; EF_ENOMEM when its buffers cannot be allocated (the context stays
  * usable). Memory: see INTEGRATION.md. Synchronises. */
 int ef_camera_create(EfContext* ctx, const EfCameraConfig* cfg, EfCamera** out);
 /* frees the camera (ef_destroy frees those still live); EF_EINVAL for a camera of another context. Synchronises. */
@@ -487,6 +505,11 @@ int ef_camera_frame_device(EfContext* ctx, EfCamera* cam, const EfCameraFrame* f
  * TIME (its prediction), FILL_* (its fill-in) and the tracker ids 40..53 without the 100*which (its pyramids, `level`). Any other id:
  * EF_EINVAL. */
 int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32_t level, void** dev_ptr, size_t* bytes);
+/* close_loops = 1: ef_local_deform_result for the camera's last frame. solved, applied and result are the camera's; deforms,
+ * last_deform_time and the graph (nodes4, n_out as there) are the context's, which the frame and its closing cameras share.
+ * EF_EINVAL for a NULL out, a negative max_nodes, NULL nodes4 with max_nodes > 0 or a camera of another context; EF_ESTATE for a
+ * camera with close_loops = 0. Synchronises. */
+int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out);
 
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
