@@ -184,6 +184,38 @@ def camera_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfCameraF
     return f
 
 
+class EfRigConfig(C.Structure):
+    _fields_ = [("n", C.c_int32), ("cameras", C.c_void_p * MAX_CAMERAS), ("T_0i", (C.c_double * 16) * MAX_CAMERAS)]
+
+
+class EfRigFrame(C.Structure):
+    _fields_ = [("time", C.c_int32), ("weight_multiplier", C.c_float), ("has_pose", C.c_int32), ("T_wc", C.c_double * 16),
+                ("fuse", C.c_int32)]
+
+
+class EfRigResult(C.Structure):
+    _fields_ = [("T_wc", C.c_double * 16), ("lastA", C.c_double * 36), ("lastb", C.c_double * 6), ("covariance", C.c_double * 36),
+                ("tracked", C.c_int32)]
+
+
+def rig_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfRigFrame:
+    """EfRigFrame: the rig's frame is stamped and predicted at `time`; T_wc (4x4 camera-to-world of member 0) sets the pose."""
+    f = EfRigFrame()
+    f.time, f.weight_multiplier, f.fuse = int(time), float(weight_multiplier), int(bool(fuse))
+    if T_wc is not None:
+        f.has_pose = 1
+        f.T_wc[:] = np.asarray(T_wc, np.float64).reshape(16).tolist()
+    return f
+
+
+def unpack_rig_result(res):
+    """(T_wc (4, 4), lastA (6, 6), lastb (6,), covariance (6, 6), tracked) of an EfRigResult or its bytes."""
+    if not isinstance(res, EfRigResult):
+        res = EfRigResult.from_buffer_copy(bytes(res))
+    return (np.array(res.T_wc[:]).reshape(4, 4), np.array(res.lastA[:]).reshape(6, 6), np.array(res.lastb[:]),
+            np.array(res.covariance[:]).reshape(6, 6), bool(res.tracked))
+
+
 def _local_deform(call):
     """(info dict, graph (n, 4) float32) of ef_local_deform_result or ef_camera_deform_result, called as call(out, nodes, n_out)"""
     res = EfLocalDeform()
@@ -662,6 +694,11 @@ class Context:
         """ef_camera_create: a camera of this context (at most MAX_CAMERAS live ones)."""
         return Camera(self, cfg)
 
+    def rig(self, cameras, extrinsics=None) -> "Rig":
+        """ef_rig_create: the cameras tracked as one rigid body; extrinsics[i] is T_0i (4x4, camera i -> cameras[0]'s camera; default:
+        identities)."""
+        return Rig(self, cameras, extrinsics)
+
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)
         _chk(lib().ef_map_upload(self.h_ctx, _p(s), len(s)))
@@ -727,3 +764,56 @@ class Camera:
         # cudaMemcpy of the CUDA runtime the library links (device to host = 2)
         _chk(lib().cudaMemcpy(_p(out), C.c_void_p(ptr), C.c_size_t(nbytes), 2))
         return out
+
+
+class Rig:
+    """One EfRig of a Context: cameras bolted together at known extrinsics, tracked as one rigid body (include/efusion_b200.h)."""
+
+    def __init__(self, ctx: Context, cameras, extrinsics=None):
+        self.ctx, self.cameras = ctx, list(cameras)
+        self.n = len(self.cameras)
+        cfg = EfRigConfig()
+        cfg.n = self.n
+        for i, cam in enumerate(self.cameras[:MAX_CAMERAS]):
+            cfg.cameras[i] = cam.h_cam.value if cam.h_cam else None
+            T = np.eye(4) if extrinsics is None else np.asarray(extrinsics[i], np.float64)
+            cfg.T_0i[i][:] = T.reshape(16).tolist()
+        self.h_rig = C.c_void_p()
+        _chk(lib().ef_rig_create(ctx.h_ctx, C.byref(cfg), C.byref(self.h_rig)))
+
+    def close(self):
+        """ef_rig_destroy (a no-op once the rig, one of its cameras or its context is closed)"""
+        if getattr(self, "h_rig", None) and self.ctx.h_ctx and all(c.h_cam for c in self.cameras):
+            _chk(lib().ef_rig_destroy(self.ctx.h_ctx, self.h_rig))
+        self.h_rig = None
+
+    def frame(self, inputs, time, weight_multiplier=1.0, T_wc=None, fuse=True, max_trace=0):
+        """ef_rig_frame: inputs[i] = (rgb (H, W, 3) uint8, depth (H, W) uint16 millimetres) of member i; T_wc (member 0's) sets the pose
+        instead of tracking. Synchronises. Returns (the members' results as Camera.frame unpacks them, each with its trace,
+        unpack_rig_result of the rig's)."""
+        arrs = []
+        for cam, (rgb, depth) in zip(self.cameras, inputs):
+            r, d = np.ascontiguousarray(rgb, np.uint8), np.ascontiguousarray(depth, np.uint16)
+            assert r.shape == (cam.h, cam.w, 3) and d.shape == (cam.h, cam.w), (r.shape, d.shape)
+            arrs.append((r, d))
+        assert len(arrs) == self.n
+        rgbs = (C.c_void_p * self.n)(*[r.ctypes.data for r, _ in arrs])
+        depths = (C.c_void_p * self.n)(*[d.ctypes.data for _, d in arrs])
+        members = (EfCameraResult * self.n)()
+        out = EfRigResult()
+        trace = np.zeros(max(max_trace, 1) * self.n, TRACE_DTYPE)
+        n_trace = (C.c_int32 * self.n)()
+        f = rig_frame(time, weight_multiplier, T_wc, fuse)
+        _chk(lib().ef_rig_frame(self.ctx.h_ctx, self.h_rig, C.byref(f), rgbs, depths, members, C.byref(out),
+                                _p(trace) if max_trace else None, int(max_trace), n_trace))
+        res = [(*unpack_camera_result(members[i]), trace[i * max_trace:i * max_trace + n_trace[i]].copy()) for i in range(self.n)]
+        return res, unpack_rig_result(out)
+
+    def frame_device(self, rgb_ptrs, depth_ptrs, members_ptr, result_ptr, time, weight_multiplier=1.0, T_wc=None, fuse=True):
+        """ef_rig_frame_device: the same from device memory into device results (members_ptr: n EfCameraResult, result_ptr: one
+        EfRigResult, 8-byte aligned), asynchronous on the context's stream."""
+        rgbs = (C.c_void_p * self.n)(*rgb_ptrs)
+        depths = (C.c_void_p * self.n)(*depth_ptrs)
+        f = rig_frame(time, weight_multiplier, T_wc, fuse)
+        _chk(lib().ef_rig_frame_device(self.ctx.h_ctx, self.h_rig, C.byref(f), rgbs, depths, C.c_void_p(members_ptr or None),
+                                       C.c_void_p(result_ptr or None)))

@@ -956,9 +956,9 @@ static bool camera_frame_ok(const EfCameraFrame* f) {
   if (f->has_pose && !finite_all(f->T_wc, 16)) return false;
   return true;
 }
-// the first frame sets the pose; fuse follows ef_map_fuse_view's rule
+// the first frame sets the pose; fuse follows ef_map_fuse_view's rule; a rig's member runs only in its rig's frames
 static int camera_frame_state(const EfContext* ctx, const EfCamera* cam, const EfCameraFrame* f) {
-  if (!cam->has_frame && !f->has_pose) return EF_ESTATE;
+  if (cam->rig || (!cam->has_frame && !f->has_pose)) return EF_ESTATE;
   return f->fuse ? fuse_view_state(ctx) : 0;
 }
 
@@ -1020,6 +1020,93 @@ extern "C" int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32
   if (dev_ptr) *dev_ptr = p;
   if (bytes) *bytes = b;
   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// rigs: cameras tracked as one rigid body (ef_track.cu, on the members' buffers and tracker slots)
+// ---------------------------------------------------------------------------------------------------------------
+// rigid and finite: |R^T R - I| <= 1e-6 entrywise and a last row of 0 0 0 1
+static bool rigid(const double* T) {
+  if (!finite_all(T, 16) || T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return false;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      double d = 0;
+      for (int k = 0; k < 3; ++k) d += T[k * 4 + i] * T[k * 4 + j];
+      if (fabs(d - (i == j ? 1.0 : 0.0)) > 1e-6) return false;
+    }
+  return true;
+}
+static bool rig_config_ok(const EfContext* ctx, const EfRigConfig* cfg) {
+  if (!cfg || cfg->n < 1 || cfg->n > EF_MAX_CAMERAS) return false;
+  const EfCamera* c0 = cfg->cameras[0];
+  for (int m = 0; m < cfg->n; ++m) {
+    const EfCamera* c = cfg->cameras[m];
+    if (!camera_of(ctx, c) || c->rig || !rigid(cfg->T_0i[m])) return false;
+    for (int j = 0; j < m; ++j)
+      if (cfg->cameras[j] == c) return false;
+    const EfCameraConfig& k = c->cfg;
+    if (k.close_loops || k.rgb_only || k.icp_weight != c0->cfg.icp_weight || k.pyramid != c0->cfg.pyramid || k.fast_odom != c0->cfg.fast_odom ||
+        k.so3 != c0->cfg.so3)
+      return false;
+  }
+  for (int k = 0; k < 16; ++k)
+    if (cfg->T_0i[0][k] != ((k % 5 == 0) ? 1.0 : 0.0)) return false;
+  return true;
+}
+static bool rig_of(const EfContext* ctx, const EfRig* rig) {
+  if (!ctx || !rig) return false;
+  for (const EfRig* r : ctx->rigs)
+    if (r == rig) return true;
+  return false;
+}
+// the camera frame's rules, once for the rig
+static int rig_frame_args(const EfContext* ctx, const EfRig* rig, const EfRigFrame* f, const void* const* rgb, const void* const* depth) {
+  if (!rig_of(ctx, rig) || !rgb || !depth) return EF_EINVAL;
+  EfCameraFrame cf = {};
+  if (f) {
+    cf.time = f->time;
+    cf.weight_multiplier = f->weight_multiplier;
+    cf.has_pose = f->has_pose;
+    memcpy(cf.T_wc, f->T_wc, sizeof(cf.T_wc));
+    cf.fuse = f->fuse;
+  }
+  if (!camera_frame_ok(f ? &cf : nullptr)) return EF_EINVAL;
+  for (int m = 0; m < rig->n; ++m)
+    if (!rgb[m] || !depth[m]) return EF_EINVAL;
+  if (!rig->has_frame && !f->has_pose) return EF_ESTATE;
+  return f->fuse ? fuse_view_state(ctx) : 0;
+}
+
+extern "C" int ef_rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out) {
+  if (!ctx || !out || !rig_config_ok(ctx, cfg)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  return rig_create(ctx, cfg, out);
+}
+extern "C" int ef_rig_destroy(EfContext* ctx, EfRig* rig) {
+  if (!rig_of(ctx, rig)) return EF_EINVAL;
+  CU(cudaSetDevice(ctx->device));
+  rig_destroy(ctx, rig);
+  return 0;
+}
+extern "C" int ef_rig_frame_device(EfContext* ctx, EfRig* rig, const EfRigFrame* f, const uint8_t* const* rgb_dev, const uint16_t* const* depth_dev,
+                                   EfCameraResult* members_dev, EfRigResult* out_dev) {
+  const int rc = rig_frame_args(ctx, rig, f, (const void* const*)rgb_dev, (const void* const*)depth_dev);
+  if (rc == EF_EINVAL || !members_dev || !out_dev || !aligned(members_dev, 8) || !aligned(out_dev, 8)) return EF_EINVAL;
+  for (int m = 0; m < rig->n; ++m)
+    if (!aligned(depth_dev[m], 2)) return EF_EINVAL;
+  RC(rc);
+  CU(cudaSetDevice(ctx->device));
+  return rig_frame_async(ctx, rig, f, rgb_dev, depth_dev, false, members_dev, out_dev);
+}
+extern "C" int ef_rig_frame(EfContext* ctx, EfRig* rig, const EfRigFrame* f, const uint8_t* const* rgb, const uint16_t* const* depth,
+                            EfCameraResult* members, EfRigResult* out, EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace) {
+  const int rc = rig_frame_args(ctx, rig, f, (const void* const*)rgb, (const void* const*)depth);
+  if (rc == EF_EINVAL || !members || !out || max_trace < 0 || (max_trace > 0 && !trace)) return EF_EINVAL;
+  RC(rc);
+  CU(cudaSetDevice(ctx->device));
+  RC(rig_frame_async(ctx, rig, f, rgb, depth, true, nullptr, nullptr));
+  RC(rig_read(ctx, rig, members, out, trace, max_trace, n_trace));  // (synchronises)
+  return ef_map_count(ctx, &ctx->host_count);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -383,6 +383,23 @@ struct LoopBuffers {
   ScanTiles scan;      // look-back tile states of the loop tracker's candidate compaction
 };
 
+// A rig's extrinsics on the device (ef_rig_*), written once at creation: T_0i (camera i -> member 0's camera), its inverse T_i0 and
+// Ad(T_i0), the adjoint that maps member 0's increment to member i's in the reference's (t, w) order: [[R, [p]x R], [0, R]], row-major
+struct RigDev {
+  double T_0i[EF_MAX_CAMERAS][16], T_i0[EF_MAX_CAMERAS][16];
+  double Ad[EF_MAX_CAMERAS][36];
+};
+// What the rig kernels (k_rig_seed, k_rig_update, k_rig_finish) work on: each member's tracker state, trace, per-level K / K^-1
+// (OdomDev::K_levels) and map pose record, in member order
+struct RigArgs {
+  int n;
+  GNState* gn[EF_MAX_CAMERAS];
+  EfSolveTrace* trace[EF_MAX_CAMERAS];
+  const double* K_levels[EF_MAX_CAMERAS];
+  MapPose* pose[EF_MAX_CAMERAS];
+  const RigDev* dev;
+};
+
 // The outcome of the last local closure of one side (the frame, or a closing camera)
 struct DeformOutcome {
   bool solved, applied;
@@ -414,6 +431,7 @@ struct EfContext {
   float odom_cam[ef::NUM_TRACKERS][4];  // level-0 {fx, fy, cx, cy} of tracker w: the host's copy of what its GNState holds
   ef::ScanTiles* odom_tiles[ef::NUM_TRACKERS];  // tile states of tracker w's candidate compaction (null: the context's own)
   EfCamera* cameras[EF_MAX_CAMERAS];           // live cameras, by tracker slot (CAMERA_TRACKER0 + i)
+  EfRig* rigs[EF_MAX_CAMERAS];                 // live rigs (each holds at least one camera)
   ef::MapDev map;
   ef::Textures tex;
   ef::Lookahead la;
@@ -475,6 +493,19 @@ struct EfCamera {
   double* pin_T;           // pinned staging of a frame's has_pose T_wc, rewritten after pose_sent
   double* dev_T;
   cudaEvent_t pose_sent;
+  EfRig* rig;              // the rig it is a member of (null: none); its own frames are refused meanwhile
+};
+
+// A rig of cameras tracked as one rigid body (ef_rig_*): its members in order (member 0's camera frame is the rig body), their
+// extrinsics and the device block the rig kernels read
+struct EfRig {
+  int n;
+  EfCamera* cams[EF_MAX_CAMERAS];
+  double T_0i[EF_MAX_CAMERAS][16];  // row-major, camera i -> member 0's camera
+  bool has_frame;                   // a first frame has set the rig's pose
+  ef::Arena arena;                  // dev and result
+  ef::RigDev* dev;
+  EfRigResult* result;              // device: the rig result of its last frame (the host call reads it back)
 };
 
 // error propagation of the host entry points: a CUDA error code, or the code of a failed internal call
@@ -589,6 +620,14 @@ int camera_frame_async(EfContext* ctx, EfCamera* cam, const EfCameraFrame* f, co
                        EfCameraResult* out_dev);
 int camera_read(EfContext* ctx, EfCamera* cam, EfCameraResult* out, EfSolveTrace* trace, int max_trace, int* n_trace);
 void camera_destroy(EfContext* ctx, EfCamera* cam);
+// ef_rig_* (include/efusion_b200.h), arguments checked by the caller: a rig of existing cameras, one rig frame (host inputs when
+// from_host; results into members_dev / out_dev when given, else into the members' and the rig's own), those own results and the
+// members' traces of its last frame (synchronises), and its release (the members stay)
+int rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out);
+int rig_frame_async(EfContext* ctx, EfRig* rig, const EfRigFrame* f, const uint8_t* const* rgb, const uint16_t* const* depth, bool from_host,
+                    EfCameraResult* members_dev, EfRigResult* out_dev);
+int rig_read(EfContext* ctx, EfRig* rig, EfCameraResult* members, EfRigResult* out, EfSolveTrace* trace, int max_trace, int* n_trace);
+void rig_destroy(EfContext* ctx, EfRig* rig);
 
 // ef_reduce.cu: SO(3) loop, Gauss-Newton schedule and the stage API's reductions
 int odom_cluster_size(int want);
@@ -601,6 +640,11 @@ int launch_se3_step_raw(EfContext* ctx, int which, int level, bool do_icp, bool 
 int launch_rgb_residual_raw(EfContext* ctx, int which, int level);
 int launch_icp_dense_only(EfContext* ctx, int which, int level);
 int launch_so3_raw(EfContext* ctx, int which);
+
+// ef_reduce.cu: a rig's joint Gauss-Newton loop over the trackers slots[0..R.n) (ef_rig_frame*; every member's model inputs, and initRGB's
+// depth half, in place), and its finish with the weighting times weightMultiplier into each member's pose record
+int rig_track_async(EfContext* ctx, const int* slots, const RigArgs& R, float icpWeight, bool pyramid, bool fastOdom, bool so3);
+int rig_finish_async(EfContext* ctx, const RigArgs& R, float weightMultiplier);
 
 // ef_preprocess.cu: filtered / metric / metric_filtered may be null
 int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,

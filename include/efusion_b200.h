@@ -511,6 +511,69 @@ int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32_t level, v
  * camera with close_loops = 0. Synchronises. */
 int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out);
 
+/* ---- rig: cameras bolted together at known extrinsics, tracked as one rigid body. A rig is built from open-loop cameras of one
+ *      context; member 0's camera frame is the rig body. One ef_rig_frame runs ef_camera_frame's steps for every member, except that
+ *      the pose is one joint estimate:
+ *        1. each member's input side and model inputs (its own fill-in choice and frame_to_frame_rgb);
+ *        2. with has_pose, member 0's pose is T_wc and member i's T_wc * T_0i; nothing is tracked. Otherwise one Gauss-Newton loop:
+ *           member 0's SO(3) pre-alignment seeds every member (resultRt_i = T_i0 * resultRt_0 * T_0i; there is no joint SO(3) solve),
+ *           then per iteration each member's systems are reduced, combined (rgb + w^2 icp), mapped into member 0's parameters through
+ *           the adjoint Ad(T_i0) (A += Ad^T A_i Ad, b += Ad^T b_i, in the (t, w) order of the update), summed and solved once; member 0
+ *           takes the update as getIncrementalTransformation would and member i is set to T_i0 * resultRt_0 * T_0i, so the rig stays
+ *           rigid at every iteration;
+ *        3. the finish: if any member's translation jumped by more than 0.3 m, every member keeps its previous pose; otherwise member 0
+ *           is orthogonalised as the tracker does and member i's pose is T_w0 * T_0i. Each member gets its own velocity weighting times
+ *           weight_multiplier;
+ *        4. with fuse, every member's map half in member order at `time`; then every member's predict() with fill-in. So each member's
+ *           next model holds the surfels the whole rig fused in this frame, which calling the cameras one after another does not give.
+ *      A one-member rig computes what ef_camera_frame computes for its camera with the context's gn_cluster off (EF_GN_CLUSTER=0); the
+ *      rig never runs the coarse levels in the cluster launch. Not covered: loop closure, rgb_only members, a joint SO(3) solve, the C++
+ *      drop-in classes and the command line.
+ *      While a camera is a member, ef_camera_frame* on it returns EF_ESTATE (ef_camera_buffer still works); ef_camera_destroy of a member
+ *      and ef_destroy free the rig first. fuse and the first frame follow the camera rules: fuse = 1 needs the context past its first
+ *      frame and not between ef_process_frame_begin and _end, and the rig's first frame must have has_pose (EF_ESTATE otherwise). A rig
+ *      may run while the look-ahead holds a staged frame and between ef_process_frame_device and ef_finish_frame (stream-ordered). */
+typedef struct EfRig EfRig;
+typedef struct {
+  int32_t n;                                /* 1..EF_MAX_CAMERAS */
+  EfCamera* cameras[EF_MAX_CAMERAS];        /* cameras of the context, each in at most one rig, with close_loops = 0, rgb_only = 0 and
+                                               the same icp_weight, pyramid, fast_odom and so3 */
+  double T_0i[EF_MAX_CAMERAS][16];          /* row-major, camera i -> member 0's camera: rigid (|R^T R - I| <= 1e-6 entrywise, last row
+                                               0 0 0 1, finite); T_0i[0] is the identity */
+} EfRigConfig;
+typedef struct {                            /* as EfCameraFrame, once for the rig */
+  int32_t time;                             /* >= 0 */
+  float weight_multiplier;                  /* finite, >= 0 */
+  int32_t has_pose;
+  double T_wc[16];                          /* member 0's pose, read when has_pose */
+  int32_t fuse;
+} EfRigFrame;
+typedef struct {
+  double T_wc[16];                          /* member 0's pose = the rig's */
+  double lastA[36], lastb[6];               /* the joint system of the last iteration, in member 0's parameters (of the last tracked
+                                               frame when this one has has_pose) */
+  double covariance[36];                    /* lastA^-1 */
+  int32_t tracked;                          /* 0 when the pose came from has_pose */
+} EfRigResult;
+/* EF_EINVAL for a NULL argument, n outside 1..EF_MAX_CAMERAS, a camera of another context or listed twice, one already in a rig, a
+ * member with close_loops or rgb_only set, members whose icp_weight, pyramid, fast_odom or so3 differ, a T_0i that is not rigid or
+ * finite, or T_0i[0] not the identity. Synchronises. */
+int ef_rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out);
+/* frees the rig; its cameras stay and may run alone again. EF_EINVAL for a rig of another context. Synchronises. */
+int ef_rig_destroy(EfContext* ctx, EfRig* rig);
+/* HOST inputs rgb[i] (RGB8, W_i*H_i*3 B) and depth[i] (uint16 millimetres) of member i; members: n results, member i's stats and
+ * covariance its own (member 0's lastA / lastb are the joint system's); synchronises. trace (HOST, may be NULL when max_trace = 0):
+ * n blocks of max_trace records, member i's at trace + i * max_trace, one per iteration of a tracked frame (member 0's SO(3) records
+ * first) with its own A_icp / A_rgb / b_icp / b_rgb, its own combined lastA / lastb and the joint result; n_trace (may be NULL): the
+ * n record counts. EF_EINVAL for a NULL argument, a rig of another context, a negative time, a bad weight_multiplier, a non-finite
+ * pose entry with has_pose, or a negative max_trace. */
+int ef_rig_frame(EfContext* ctx, EfRig* rig, const EfRigFrame* frame, const uint8_t* const* rgb, const uint16_t* const* depth,
+                 EfCameraResult* members, EfRigResult* out, EfSolveTrace* trace, int32_t max_trace, int32_t* n_trace);
+/* same from DEVICE inputs into DEVICE results (members_dev: n EfCameraResult), asynchronous on ef_stream(); EF_EINVAL also for a
+ * depth pointer not aligned to 2 bytes or a result not aligned to 8 */
+int ef_rig_frame_device(EfContext* ctx, EfRig* rig, const EfRigFrame* frame, const uint8_t* const* rgb_dev, const uint16_t* const* depth_dev,
+                        EfCameraResult* members_dev, EfRigResult* out_dev);
+
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
   /* input / preprocess textures (ElasticFusion::textures, GPUTexture.cpp:22-27) */
