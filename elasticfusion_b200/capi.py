@@ -198,6 +198,12 @@ class EfRigResult(C.Structure):
                 ("tracked", C.c_int32)]
 
 
+class EfRigLoopResult(C.Structure):
+    _fields_ = [("ran", C.c_int32), ("accepted", C.c_int32), ("n_constraints", C.c_int32), ("member_constraints", C.c_int32 * MAX_CAMERAS),
+                ("lastICPError", C.c_float), ("lastICPCount", C.c_float), ("cov_diag", C.c_double * 6), ("T_wc_curr", C.c_double * 16),
+                ("T_wc_est", C.c_double * 16)]
+
+
 def rig_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfRigFrame:
     """EfRigFrame: the rig's frame is stamped and predicted at `time`; T_wc (4x4 camera-to-world of member 0) sets the pose."""
     f = EfRigFrame()
@@ -817,3 +823,24 @@ class Rig:
         f = rig_frame(time, weight_multiplier, T_wc, fuse)
         _chk(lib().ef_rig_frame_device(self.ctx.h_ctx, self.h_rig, C.byref(f), rgbs, depths, C.c_void_p(members_ptr or None),
                                        C.c_void_p(result_ptr or None)))
+
+    def loop_result(self):
+        """A closing rig: (info dict, src (n,3), dst (n,3), times (n,), member_counts (n_members,)) of its last frame's front half, as
+        Context.local_loop_result returns the frame's; the constraints are the members', concatenated in member order."""
+        res = EfRigLoopResult()
+        cap = sum((c.w // 20) * (c.h // 20) for c in self.cameras)
+        src = np.zeros((cap, 3), np.float64)
+        dst = np.zeros((cap, 3), np.float64)
+        tm = np.zeros(cap, np.int32)
+        n = C.c_int32()
+        _chk(lib().ef_rig_loop_result(self.ctx.h_ctx, self.h_rig, C.byref(res), _p(src), _p(dst), _p(tm), cap, C.byref(n)))
+        info = dict(ran=res.ran, accepted=res.accepted, n_constraints=res.n_constraints, lastICPError=res.lastICPError,
+                    lastICPCount=res.lastICPCount, cov_diag=np.array(res.cov_diag[:]), T_wc_curr=np.array(res.T_wc_curr[:]).reshape(4, 4),
+                    T_wc_est=np.array(res.T_wc_est[:]).reshape(4, 4))
+        counts = np.array(res.member_constraints[:self.n], np.int32)
+        return info, src[:n.value].copy(), dst[:n.value].copy(), tm[:n.value].copy(), counts
+
+    def deform_result(self):
+        """A closing rig: (info dict, graph) of its last frame, as Camera.deform_result returns them (solved, applied and result are
+        the rig's; deforms, last_deform_time and the graph the context's)."""
+        return _local_deform(lambda res, nodes, n: lib().ef_rig_deform_result(self.ctx.h_ctx, self.h_rig, res, _p(nodes), len(nodes), n))

@@ -1045,7 +1045,7 @@ static bool rig_config_ok(const EfContext* ctx, const EfRigConfig* cfg) {
     for (int j = 0; j < m; ++j)
       if (cfg->cameras[j] == c) return false;
     const EfCameraConfig& k = c->cfg;
-    if (k.close_loops || k.rgb_only || k.icp_weight != c0->cfg.icp_weight || k.pyramid != c0->cfg.pyramid || k.fast_odom != c0->cfg.fast_odom ||
+    if (k.close_loops != c0->cfg.close_loops || k.rgb_only || k.icp_weight != c0->cfg.icp_weight || k.pyramid != c0->cfg.pyramid || k.fast_odom != c0->cfg.fast_odom ||
         k.so3 != c0->cfg.so3)
       return false;
   }
@@ -1254,13 +1254,17 @@ namespace ef {
 // made: modelToModel in the reference's order (initICPModel -> initRGBModel -> initICP(pred, pred) -> initRGB, App. A-2),
 // getIncrementalTransformation(rgbOnly = false, icpWeight = 10, so3 = false), acceptance test and constraint sampling.
 // Everything stays on the device (LoopDev); nothing is applied to the map or the pose.
-int loop_front_half(EfContext* ctx, const LoopSide& s) {
+int loop_tracker_inputs(EfContext* ctx, const LoopSide& s) {
   OdomDev& od = ctx->odom[s.est];
   RC(odom_copy_pose_async(ctx, s.est, s.curr));
   RC(odom_init_icp_model(ctx, s.est, (const float*)s.old_vertex, (const float*)s.old_normal, false));
   RC(odom_populate(ctx, s.est, (const uint8_t*)s.old_image, od.lastDepth, od.lastImage, true));
   RC(odom_init_icp_pred(ctx, s.est, (const float*)s.vertex, (const float*)s.normal));
-  RC(odom_populate(ctx, s.est, (const uint8_t*)s.image, od.nextDepth, od.nextImage, true));
+  return odom_populate(ctx, s.est, (const uint8_t*)s.image, od.nextDepth, od.nextImage, true);
+}
+
+int loop_front_half(EfContext* ctx, const LoopSide& s) {
+  RC(loop_tracker_inputs(ctx, s));
   RC(odom_track_async(ctx, s.est, false, 10.0f, s.pyramid, s.fast_odom, false));
   RC(odom_finish_async(ctx, s.est, 1.0f, true, nullptr));
   return map_loop_constraints_async(ctx, s);
@@ -1495,9 +1499,48 @@ extern "C" int ef_local_deform_result(EfContext* ctx, EfLocalDeform* out, float*
 
 extern "C" int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out) {
   if (!camera_of(ctx, cam) || !out || max_nodes < 0 || (max_nodes > 0 && !nodes4)) return EF_EINVAL;
-  if (!cam->cfg.close_loops) return EF_ESTATE;
+  if (!cam->cfg.close_loops || cam->rig) return EF_ESTATE;
   CU(cudaSetDevice(ctx->device));
   return deform_report(ctx, cam->deform_out, out, nodes4, max_nodes, n_out);
+}
+
+extern "C" int ef_rig_deform_result(EfContext* ctx, EfRig* rig, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out) {
+  if (!rig_of(ctx, rig) || !out || max_nodes < 0 || (max_nodes > 0 && !nodes4)) return EF_EINVAL;
+  if (!rig->closing) return EF_ESTATE;
+  CU(cudaSetDevice(ctx->device));
+  return deform_report(ctx, rig->deform_out, out, nodes4, max_nodes, n_out);
+}
+
+extern "C" int ef_rig_loop_result(EfContext* ctx, EfRig* rig, EfRigLoopResult* out, double* src3, double* dst3, int32_t* times,
+                                  int32_t max_constraints, int32_t* n_out) {
+  if (!rig_of(ctx, rig) || !out || max_constraints < 0) return EF_EINVAL;
+  if (!rig->closing) return EF_ESTATE;
+  CU(cudaSetDevice(ctx->device));
+  LoopDev h;
+  RigLoopDev rec;
+  CU(cudaMemcpyAsync(&h, rig->loop, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&rec, rig->loop_rec, sizeof(rec), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  memset(out, 0, sizeof(*out));
+  out->ran = h.ran;
+  out->accepted = h.accepted;
+  out->n_constraints = h.n_constraints;
+  for (int m = 0; m < EF_MAX_CAMERAS; ++m) out->member_constraints[m] = rec.member_n[m];
+  out->lastICPError = h.lastICPError;
+  out->lastICPCount = h.lastICPCount;
+  memcpy(out->cov_diag, h.cov_diag, sizeof(h.cov_diag));
+  memcpy(out->T_wc_curr, rec.T_wc_curr, sizeof(rec.T_wc_curr));
+  memcpy(out->T_wc_est, h.T_wc_est, sizeof(h.T_wc_est));
+  int n = h.n_constraints < max_constraints ? h.n_constraints : max_constraints;
+  if (n > rig->capacity) n = rig->capacity;
+  if (n_out) *n_out = n;
+  if (n > 0) {
+    if (src3) CU(cudaMemcpyAsync(src3, rig->src, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (dst3) CU(cudaMemcpyAsync(dst3, rig->dst, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (times) CU(cudaMemcpyAsync(times, rig->times, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
 }
 
 extern "C" int ef_local_loop_result(EfContext* ctx, EfLoopResult* out, double* src3, double* dst3, int32_t* times, int32_t max_constraints,

@@ -384,20 +384,46 @@ struct LoopBuffers {
 };
 
 // A rig's extrinsics on the device (ef_rig_*), written once at creation: T_0i (camera i -> member 0's camera), its inverse T_i0 and
-// Ad(T_i0), the adjoint that maps member 0's increment to member i's in the reference's (t, w) order: [[R, [p]x R], [0, R]], row-major
+// Ad(T_i0), the adjoint that maps member 0's increment to member i's in the reference's (t, w) order: [[R, [p]x R], [0, R]], row-major.
+// res: each member's ICP residual sum and inlier count of the last iteration (res0, res1 of gn_gather), written by k_rig_update.
 struct RigDev {
   double T_0i[EF_MAX_CAMERAS][16], T_i0[EF_MAX_CAMERAS][16];
   double Ad[EF_MAX_CAMERAS][36];
+  float res[EF_MAX_CAMERAS][2];
 };
 // What the rig kernels (k_rig_seed, k_rig_update, k_rig_finish) work on: each member's tracker state, trace, per-level K / K^-1
-// (OdomDev::K_levels) and map pose record, in member order
+// (OdomDev::K_levels) and map pose record (null: none), in member order
 struct RigArgs {
   int n;
   GNState* gn[EF_MAX_CAMERAS];
   EfSolveTrace* trace[EF_MAX_CAMERAS];
   const double* K_levels[EF_MAX_CAMERAS];
   MapPose* pose[EF_MAX_CAMERAS];
+  RigDev* dev;
+};
+
+// A closing rig's record of its last front half besides its LoopDev: each member's constraint count and member 0's T_wc_curr
+struct RigLoopDev {
+  int member_n[EF_MAX_CAMERAS];
+  double T_wc_curr[16];
+};
+// What k_rig_loop_constraints works on: each member's tracker (T_wc_curr) and loop tracker after the joint model-to-model
+// registration (T_wc_est; member 0's lastA is the joint system), its ACTIVE prediction and INACTIVE time stamps at its size, the
+// members' residuals (RigDev::res) and the rig's record and constraint buffers (capacity: the sum of the members' grids)
+struct RigLoopArgs {
+  int n;
+  const GNState* curr[EF_MAX_CAMERAS];
+  const GNState* est[EF_MAX_CAMERAS];
+  const float4* vertex[EF_MAX_CAMERAS];
+  const uint16_t* old_time[EF_MAX_CAMERAS];
+  int rows[EF_MAX_CAMERAS], cols[EF_MAX_CAMERAS];
+  float max_depth[EF_MAX_CAMERAS];
   const RigDev* dev;
+  LoopDev* loop;
+  RigLoopDev* rec;
+  double *src, *dst;
+  int* times;
+  int capacity;
 };
 
 // The outcome of the last local closure of one side (the frame, or a closing camera)
@@ -503,9 +529,17 @@ struct EfRig {
   EfCamera* cams[EF_MAX_CAMERAS];
   double T_0i[EF_MAX_CAMERAS][16];  // row-major, camera i -> member 0's camera
   bool has_frame;                   // a first frame has set the rig's pose
-  ef::Arena arena;                  // dev and result
+  ef::Arena arena;                  // dev, result and a closing rig's loop buffers
   ef::RigDev* dev;
   EfRigResult* result;              // device: the rig result of its last frame (the host call reads it back)
+  // every member has close_loops = 1: the rig closes local loops as one body (its members' loop trackers and LoopBuffers, and these)
+  bool closing;
+  ef::LoopDev* loop;
+  ef::RigLoopDev* loop_rec;
+  double *src, *dst;                // the members' constraints, concatenated in member order
+  int* times;
+  int capacity;                     // the sum of the members' loop_constraint_capacity
+  ef::DeformOutcome deform_out;     // its last frame's closure
 };
 
 // error propagation of the host entry points: a CUDA error code, or the code of a failed internal call
@@ -596,6 +630,8 @@ int alloc_odom(EfContext* ctx, Arena& arena, int which, int width, int height, f
 // 457-505); loop_solve_apply: the read-back, solve and hand-over (:505-526) at `time`, the pose going to tracker s.curr and pose_record;
 // *n_nodes: the graph the clean applies (0: none)
 int loop_front_half(EfContext* ctx, const LoopSide& s);
+// its first steps: tracker s.est at the pose of s.curr with the INACTIVE prediction as its model and the ACTIVE one as its input
+int loop_tracker_inputs(EfContext* ctx, const LoopSide& s);
 int loop_solve_apply(EfContext* ctx, const LoopSide& s, int time, MapPose* pose_record, DeformOutcome* out, int* n_nodes);
 
 // ef_track.cu: the tracker's input pyramids
@@ -645,6 +681,8 @@ int launch_so3_raw(EfContext* ctx, int which);
 // depth half, in place), and its finish with the weighting times weightMultiplier into each member's pose record
 int rig_track_async(EfContext* ctx, const int* slots, const RigArgs& R, float icpWeight, bool pyramid, bool fastOdom, bool so3);
 int rig_finish_async(EfContext* ctx, const RigArgs& R, float weightMultiplier);
+// after a closure set member 0's pose: member i's T_wc = T_w0 * T_0i in double, and its pose record
+int rig_apply_pose_async(EfContext* ctx, const RigArgs& R);
 
 // ef_preprocess.cu: filtered / metric / metric_filtered may be null
 int preprocess_depth(EfContext* ctx, int rows, int cols, const uint16_t* raw, float cutoff, uint16_t* filtered, float* metric,
@@ -697,6 +735,8 @@ int map_predict_target_async(EfContext* ctx, const PredictTarget& t, float max_d
 int map_dense_enough_async(EfContext* ctx);
 // the acceptance test and the constraints of side s's front half, with the context's thresholds
 int map_loop_constraints_async(EfContext* ctx, const LoopSide& s);
+// the same for a closing rig: one joint acceptance test and every member's grid, concatenated in member order
+int map_rig_loop_constraints_async(EfContext* ctx, const RigLoopArgs& a);
 int map_loop_reset_async(EfContext* ctx, LoopDev* loop);
 // the map kernels' pose record `mp` from a device T_wc
 int map_pose_record_async(EfContext* ctx, MapPose* mp, const double* T_dev);

@@ -511,9 +511,9 @@ int ef_camera_buffer(EfContext* ctx, EfCamera* cam, int32_t id, int32_t level, v
  * camera with close_loops = 0. Synchronises. */
 int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out);
 
-/* ---- rig: cameras bolted together at known extrinsics, tracked as one rigid body. A rig is built from open-loop cameras of one
- *      context; member 0's camera frame is the rig body. One ef_rig_frame runs ef_camera_frame's steps for every member, except that
- *      the pose is one joint estimate:
+/* ---- rig: cameras bolted together at known extrinsics, tracked as one rigid body. A rig is built from cameras of one context that
+ *      all have close_loops = 0 (an open-loop rig) or all close_loops = 1 (a closing rig); member 0's camera frame is the rig body. One
+ *      ef_rig_frame runs ef_camera_frame's steps for every member, except that the pose is one joint estimate:
  *        1. each member's input side and model inputs (its own fill-in choice and frame_to_frame_rgb);
  *        2. with has_pose, member 0's pose is T_wc and member i's T_wc * T_0i; nothing is tracked. Otherwise one Gauss-Newton loop:
  *           member 0's SO(3) pre-alignment seeds every member (resultRt_i = T_i0 * resultRt_0 * T_0i; there is no joint SO(3) solve),
@@ -527,17 +527,37 @@ int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, f
  *        4. with fuse, every member's map half in member order at `time`; then every member's predict() with fill-in. So each member's
  *           next model holds the surfels the whole rig fused in this frame, which calling the cameras one after another does not give.
  *      A one-member rig computes what ef_camera_frame computes for its camera with the context's gn_cluster off (EF_GN_CLUSTER=0); the
- *      rig never runs the coarse levels in the cluster launch. Not covered: loop closure, rgb_only members, a joint SO(3) solve, the C++
- *      drop-in classes and the command line.
- *      While a camera is a member, ef_camera_frame* on it returns EF_ESTATE (ef_camera_buffer still works); ef_camera_destroy of a member
+ *      rig never runs the coarse levels in the cluster launch. Not covered: rgb_only members, a joint SO(3) solve, the C++ drop-in
+ *      classes and the command line.
+ *
+ *      A closing rig closes local loops as one body, on the context's graph (T_x_i = T_x_0 * T_0i throughout):
+ *        - on a fused frame after the rig's first (has_pose frames too), after step 3: each member's predict() ACTIVE at (time, time,
+ *          time_delta) and INACTIVE prediction at (0, time - time_delta, time_delta), as a closing camera makes them; each member's loop
+ *          tracker at its pose, with the INACTIVE prediction as its model; one joint model-to-model registration over the members' loop
+ *          trackers (step 2's solve with rgb_only = 0, icp_weight = 10, no SO(3)) and step 3's finish, so T_est_i = T_est_0 * T_0i;
+ *        - one acceptance test: every diagonal entry of the joint system's inverse within cov_thresh, count > count_thresh and
+ *          error < err_thresh, where count is the ICP inlier count SUMMED over the members and error = sqrt(sum of their ICP
+ *          residuals) / count (for one member, the camera's test);
+ *        - accepted, each member's (W_i/20) x (H_i/20) grid is sampled as a closing camera samples its own (src = T_curr_i v,
+ *          dst = T_est_i v, time = its INACTIVE stamp), concatenated in member order; with a graph and a constraint, one solve of
+ *          them all (pin = (deforms == 0), source time `time`) and, unless it stops with code 6, member 0's pose becomes T_est_0 and
+ *          member i's T_est_0 * T_0i; only member 0's clean in step 4 deforms the map (the map is deformed once); then deforms += 1
+ *          and last_deform_time = time;
+ *        - at the end of every call, the graph is sampled from the map (fuse = 0 and first calls too).
+ *      The members' EfCameraResult.T_wc and EfRigResult.T_wc are then the closed poses; the weighting is the one computed before the
+ *      closure. ef_rig_frame_device waits for the host once for the front half's record and, on a frame that solves, once more for
+ *      the solve (as a closing camera does). Results: ef_rig_loop_result and ef_rig_deform_result. A one-member closing rig computes
+ *      what its closing camera computes with gn_cluster off.
+ *      While a camera is a member, ef_camera_frame* and ef_camera_deform_result on it return EF_ESTATE (ef_camera_buffer still works);
+ *      after ef_rig_destroy its members run alone again (a closing camera closes its own loops). ef_camera_destroy of a member
  *      and ef_destroy free the rig first. fuse and the first frame follow the camera rules: fuse = 1 needs the context past its first
  *      frame and not between ef_process_frame_begin and _end, and the rig's first frame must have has_pose (EF_ESTATE otherwise). A rig
  *      may run while the look-ahead holds a staged frame and between ef_process_frame_device and ef_finish_frame (stream-ordered). */
 typedef struct EfRig EfRig;
 typedef struct {
   int32_t n;                                /* 1..EF_MAX_CAMERAS */
-  EfCamera* cameras[EF_MAX_CAMERAS];        /* cameras of the context, each in at most one rig, with close_loops = 0, rgb_only = 0 and
-                                               the same icp_weight, pyramid, fast_odom and so3 */
+  EfCamera* cameras[EF_MAX_CAMERAS];        /* cameras of the context, each in at most one rig, with rgb_only = 0 and the same
+                                               close_loops, icp_weight, pyramid, fast_odom and so3 */
   double T_0i[EF_MAX_CAMERAS][16];          /* row-major, camera i -> member 0's camera: rigid (|R^T R - I| <= 1e-6 entrywise, last row
                                                0 0 0 1, finite); T_0i[0] is the identity */
 } EfRigConfig;
@@ -556,8 +576,9 @@ typedef struct {
   int32_t tracked;                          /* 0 when the pose came from has_pose */
 } EfRigResult;
 /* EF_EINVAL for a NULL argument, n outside 1..EF_MAX_CAMERAS, a camera of another context or listed twice, one already in a rig, a
- * member with close_loops or rgb_only set, members whose icp_weight, pyramid, fast_odom or so3 differ, a T_0i that is not rigid or
- * finite, or T_0i[0] not the identity. Synchronises. */
+ * member with rgb_only set, members whose close_loops, icp_weight, pyramid, fast_odom or so3 differ, a T_0i that is not rigid or
+ * finite, or T_0i[0] not the identity. EF_ENOMEM when a closing rig's buffers cannot be allocated (the context stays usable).
+ * Synchronises. */
 int ef_rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out);
 /* frees the rig; its cameras stay and may run alone again. EF_EINVAL for a rig of another context. Synchronises. */
 int ef_rig_destroy(EfContext* ctx, EfRig* rig);
@@ -573,6 +594,26 @@ int ef_rig_frame(EfContext* ctx, EfRig* rig, const EfRigFrame* frame, const uint
  * depth pointer not aligned to 2 bytes or a result not aligned to 8 */
 int ef_rig_frame_device(EfContext* ctx, EfRig* rig, const EfRigFrame* frame, const uint8_t* const* rgb_dev, const uint16_t* const* depth_dev,
                         EfCameraResult* members_dev, EfRigResult* out_dev);
+/* a closing rig's front half of its last frame, as EfLoopResult reports the frame's */
+typedef struct {
+  int32_t ran;                                   /* 0: no front half ran (a first or fuse = 0 call) */
+  int32_t accepted;                              /* the joint test (see above) */
+  int32_t n_constraints;                         /* the sum of member_constraints */
+  int32_t member_constraints[EF_MAX_CAMERAS];    /* each member's, at most its (W_i/20) x (H_i/20) grid (0 beyond n) */
+  float lastICPError, lastICPCount;              /* the joint error and the summed count the test compared */
+  double cov_diag[6];                            /* of the joint system's inverse */
+  double T_wc_curr[16];                          /* member 0's pose before the closure */
+  double T_wc_est[16];                           /* member 0's pose after the joint registration */
+} EfRigLoopResult;
+/* ef_local_loop_result for a closing rig's last frame: src3 / dst3 / times (HOST, any may be NULL) receive the concatenated
+ * constraints, at most max_constraints; n_out (may be NULL) their number. EF_EINVAL for a NULL out, a negative max_constraints or a
+ * rig of another context; EF_ESTATE for an open-loop rig. Synchronises. */
+int ef_rig_loop_result(EfContext* ctx, EfRig* rig, EfRigLoopResult* out, double* src3, double* dst3, int32_t* times, int32_t max_constraints,
+                       int32_t* n_out);
+/* ef_camera_deform_result for a closing rig's last frame: solved, applied and result are the rig's; deforms, last_deform_time and the
+ * graph the context's. EF_EINVAL for a NULL out, a negative max_nodes, NULL nodes4 with max_nodes > 0 or a rig of another context;
+ * EF_ESTATE for an open-loop rig. Synchronises. */
+int ef_rig_deform_result(EfContext* ctx, EfRig* rig, EfLocalDeform* out, float* nodes4, int32_t max_nodes, int32_t* n_out);
 
 /* ---- named device buffers (the reference's GPUTexture / DeviceArray handles) ------------------------------ */
 enum {
