@@ -185,7 +185,7 @@ def camera_frame(time, weight_multiplier=1.0, T_wc=None, fuse=True) -> EfCameraF
 
 
 class EfRigConfig(C.Structure):
-    _fields_ = [("n", C.c_int32), ("cameras", C.c_void_p * MAX_CAMERAS), ("T_0i", (C.c_double * 16) * MAX_CAMERAS)]
+    _fields_ = [("n", C.c_int32), ("cameras", C.c_void_p * MAX_CAMERAS), ("T_0i", (C.c_double * 16) * MAX_CAMERAS), ("joint_so3", C.c_int32)]
 
 
 class EfRigFrame(C.Structure):
@@ -700,10 +700,10 @@ class Context:
         """ef_camera_create: a camera of this context (at most MAX_CAMERAS live ones)."""
         return Camera(self, cfg)
 
-    def rig(self, cameras, extrinsics=None) -> "Rig":
+    def rig(self, cameras, extrinsics=None, joint_so3=False) -> "Rig":
         """ef_rig_create: the cameras tracked as one rigid body; extrinsics[i] is T_0i (4x4, camera i -> cameras[0]'s camera; default:
-        identities)."""
-        return Rig(self, cameras, extrinsics)
+        identities); joint_so3: one SO(3) pre-alignment over every member's images instead of member 0's."""
+        return Rig(self, cameras, extrinsics, joint_so3)
 
     def map_upload(self, surfels):
         s = np.ascontiguousarray(surfels, np.float32)
@@ -775,11 +775,12 @@ class Camera:
 class Rig:
     """One EfRig of a Context: cameras bolted together at known extrinsics, tracked as one rigid body (include/efusion_b200.h)."""
 
-    def __init__(self, ctx: Context, cameras, extrinsics=None):
+    def __init__(self, ctx: Context, cameras, extrinsics=None, joint_so3=False):
         self.ctx, self.cameras = ctx, list(cameras)
         self.n = len(self.cameras)
         cfg = EfRigConfig()
         cfg.n = self.n
+        cfg.joint_so3 = 1 if joint_so3 else 0
         for i, cam in enumerate(self.cameras[:MAX_CAMERAS]):
             cfg.cameras[i] = cam.h_cam.value if cam.h_cam else None
             T = np.eye(4) if extrinsics is None else np.asarray(extrinsics[i], np.float64)

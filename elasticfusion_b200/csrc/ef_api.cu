@@ -1037,7 +1037,7 @@ static bool rigid(const double* T) {
   return true;
 }
 static bool rig_config_ok(const EfContext* ctx, const EfRigConfig* cfg) {
-  if (!cfg || cfg->n < 1 || cfg->n > EF_MAX_CAMERAS) return false;
+  if (!cfg || cfg->n < 1 || cfg->n > EF_MAX_CAMERAS || (cfg->joint_so3 != 0 && cfg->joint_so3 != 1)) return false;
   const EfCamera* c0 = cfg->cameras[0];
   for (int m = 0; m < cfg->n; ++m) {
     const EfCamera* c = cfg->cameras[m];
@@ -1046,7 +1046,7 @@ static bool rig_config_ok(const EfContext* ctx, const EfRigConfig* cfg) {
       if (cfg->cameras[j] == c) return false;
     const EfCameraConfig& k = c->cfg;
     if (k.close_loops != c0->cfg.close_loops || k.rgb_only || k.icp_weight != c0->cfg.icp_weight || k.pyramid != c0->cfg.pyramid || k.fast_odom != c0->cfg.fast_odom ||
-        k.so3 != c0->cfg.so3)
+        k.so3 != c0->cfg.so3 || (cfg->joint_so3 && !k.so3))
       return false;
   }
   for (int k = 0; k < 16; ++k)

@@ -401,6 +401,21 @@ struct RigArgs {
   MapPose* pose[EF_MAX_CAMERAS];
   RigDev* dev;
 };
+// What a rig's joint SO(3) pre-alignment (k_rig_so3_begin, k_rig_so3_step) works on: each member's SO(3) state, the GNState whose
+// level-2 K its homography uses, its level-2 image pair and size and its partials; member m's CTAs are [cta0[m], cta0[m + 1]). The
+// extrinsics are the rig's; the ticket, the rig's own, replaces the members' so3_counter.
+struct RigSo3Args {
+  int n;
+  So3State* so3[EF_MAX_CAMERAS];
+  const GNState* gn[EF_MAX_CAMERAS];
+  const uint8_t* last[EF_MAX_CAMERAS];
+  const uint8_t* next[EF_MAX_CAMERAS];
+  int rows[EF_MAX_CAMERAS], cols[EF_MAX_CAMERAS];
+  float* partials[EF_MAX_CAMERAS];
+  int cta0[EF_MAX_CAMERAS + 1];
+  const RigDev* dev;
+  unsigned int* ticket;
+};
 
 // A closing rig's record of its last front half besides its LoopDev: each member's constraint count and member 0's T_wc_curr
 struct RigLoopDev {
@@ -540,6 +555,9 @@ struct EfRig {
   int* times;
   int capacity;                     // the sum of the members' loop_constraint_capacity
   ef::DeformOutcome deform_out;     // its last frame's closure
+  // joint_so3: one SO(3) pre-alignment over every member's image pair instead of member 0's; the ticket of its reduction
+  bool joint_so3;
+  unsigned int* so3_ticket;
 };
 
 // error propagation of the host entry points: a CUDA error code, or the code of a failed internal call
@@ -678,8 +696,10 @@ int launch_icp_dense_only(EfContext* ctx, int which, int level);
 int launch_so3_raw(EfContext* ctx, int which);
 
 // ef_reduce.cu: a rig's joint Gauss-Newton loop over the trackers slots[0..R.n) (ef_rig_frame*; every member's model inputs, and initRGB's
-// depth half, in place), and its finish with the weighting times weightMultiplier into each member's pose record
-int rig_track_async(EfContext* ctx, const int* slots, const RigArgs& R, float icpWeight, bool pyramid, bool fastOdom, bool so3);
+// depth half, in place), and its finish with the weighting times weightMultiplier into each member's pose record. so3_ticket (the
+// rig's, zero between launches): the SO(3) pre-alignment is the joint one over every member (null: member 0's)
+int rig_track_async(EfContext* ctx, const int* slots, const RigArgs& R, float icpWeight, bool pyramid, bool fastOdom, bool so3,
+                    unsigned int* so3_ticket);
 int rig_finish_async(EfContext* ctx, const RigArgs& R, float weightMultiplier);
 // after a closure set member 0's pose: member i's T_wc = T_w0 * T_0i in double, and its pose record
 int rig_apply_pose_async(EfContext* ctx, const RigArgs& R);

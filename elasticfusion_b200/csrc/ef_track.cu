@@ -1159,11 +1159,13 @@ static void rig_adjoint(const double* T, double* Ad) {
     }
 }
 
-// the rig's device block (host's extrinsics), its result and, for a closing rig, its loop record and concatenated constraint buffers
+// the rig's device block (host's extrinsics), its result, the ticket of a joint SO(3) pre-alignment and, for a closing rig, its loop
+// record and concatenated constraint buffers
 static int rig_alloc(EfContext* ctx, EfRig* r, const RigDev& host) {
   CU(arena_alloc(ctx, r->arena, &r->dev, 1));
   CU(arena_alloc(ctx, r->arena, &r->result, 1, 0));
   CU(cudaMemcpyAsync(r->dev, &host, sizeof(host), cudaMemcpyHostToDevice, ctx->stream));
+  if (r->joint_so3) CU(arena_alloc(ctx, r->arena, &r->so3_ticket, 1, 0));
   if (r->closing) {
     CU(arena_alloc(ctx, r->arena, &r->loop, 1, 0));
     CU(arena_alloc(ctx, r->arena, &r->loop_rec, 1, 0));
@@ -1191,6 +1193,7 @@ int rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out) {
     rig_adjoint(host.T_i0[m], host.Ad[m]);
   }
   r->closing = r->cams[0]->cfg.close_loops != 0;  // (ef_rig_create checks that every member agrees)
+  r->joint_so3 = cfg->joint_so3 != 0;
   for (int m = 0; m < r->n && r->closing; ++m) r->capacity += r->cams[m]->loop.capacity;
   int rc = rig_alloc(ctx, r, host);
   if (rc) {
@@ -1267,7 +1270,7 @@ static int rig_close_loop(EfContext* ctx, EfRig* r, int time, EfCameraResult* co
     a.max_depth[m] = s.max_depth;
   }
   const EfCameraConfig& k = r->cams[0]->cfg;
-  RC(rig_track_async(ctx, slots, L, 10.0f, k.pyramid != 0, k.fast_odom != 0, false));
+  RC(rig_track_async(ctx, slots, L, 10.0f, k.pyramid != 0, k.fast_odom != 0, false, nullptr));
   RC(rig_finish_async(ctx, L, 1.0f));
   RC(map_rig_loop_constraints_async(ctx, a));
   LoopSide s = {};  // what loop_solve_apply reads: the record, the constraints and member 0's tracker
@@ -1320,7 +1323,7 @@ int rig_frame_async(EfContext* ctx, EfRig* r, const EfRigFrame* f, const uint8_t
       mi[ready] = camera_model_inputs(r->cams[ready]);
       rc = track_model_side(ctx, slots[ready], mi[ready], saved[ready]);
     }
-    if (!rc) rc = rig_track_async(ctx, slots, R, k.icp_weight, k.pyramid != 0, k.fast_odom != 0, k.so3 != 0);
+    if (!rc) rc = rig_track_async(ctx, slots, R, k.icp_weight, k.pyramid != 0, k.fast_odom != 0, k.so3 != 0, r->joint_so3 ? r->so3_ticket : nullptr);
     for (int m = 0; m < ready; ++m) track_model_restore(ctx, slots[m], mi[m], saved[m]);
     RC(rc);
     RC(rig_finish_async(ctx, R, f->weight_multiplier));

@@ -516,19 +516,24 @@ int ef_camera_deform_result(EfContext* ctx, EfCamera* cam, EfLocalDeform* out, f
  *      ef_rig_frame runs ef_camera_frame's steps for every member, except that the pose is one joint estimate:
  *        1. each member's input side and model inputs (its own fill-in choice and frame_to_frame_rgb);
  *        2. with has_pose, member 0's pose is T_wc and member i's T_wc * T_0i; nothing is tracked. Otherwise one Gauss-Newton loop:
- *           member 0's SO(3) pre-alignment seeds every member (resultRt_i = T_i0 * resultRt_0 * T_0i; there is no joint SO(3) solve),
- *           then per iteration each member's systems are reduced, combined (rgb + w^2 icp), mapped into member 0's parameters through
+ *           the SO(3) pre-alignment seeds every member (resultRt_i = T_i0 * resultRt_0 * T_0i), then per iteration each member's systems are reduced, combined (rgb + w^2 icp), mapped into member 0's parameters through
  *           the adjoint Ad(T_i0) (A += Ad^T A_i Ad, b += Ad^T b_i, in the (t, w) order of the update), summed and solved once; member 0
  *           takes the update as getIncrementalTransformation would and member i is set to T_i0 * resultRt_0 * T_0i, so the rig stays
- *           rigid at every iteration;
+ *           rigid at every iteration. The pre-alignment is member 0's alone, or with joint_so3 one loop for the whole body: member
+ *           0's loop state is the body's and member i's rotation is R_i0 * R_0 * R_0i; per iteration each member reduces its own
+ *           level-2 image pair at its own homography, member i's 3x3 system enters the joint one as R_0i A_i R_0i^T, R_0i b_i (sums
+ *           in double, then float), the error is sqrt(sum of res0) / sum of res1 and the count the sum of res1, and the reference's
+ *           convergence and divergence tests and update act on these for member 0 (on divergence every member keeps its last
+ *           rotation); every member reports the joint SO(3) error and count. A one-member joint rig computes what its camera computes
+ *           with gn_cluster off, except for the joint fields of its SO(3) trace records;
  *        3. the finish: if any member's translation jumped by more than 0.3 m, every member keeps its previous pose; otherwise member 0
  *           is orthogonalised as the tracker does and member i's pose is T_w0 * T_0i. Each member gets its own velocity weighting times
  *           weight_multiplier;
  *        4. with fuse, every member's map half in member order at `time`; then every member's predict() with fill-in. So each member's
  *           next model holds the surfels the whole rig fused in this frame, which calling the cameras one after another does not give.
  *      A one-member rig computes what ef_camera_frame computes for its camera with the context's gn_cluster off (EF_GN_CLUSTER=0); the
- *      rig never runs the coarse levels in the cluster launch. Not covered: rgb_only members, a joint SO(3) solve, the C++ drop-in
- *      classes and the command line.
+ *      rig never runs the coarse levels in the cluster launch, nor the SO(3) pre-alignment when it is joint. Not covered: rgb_only
+ *      members, the C++ drop-in classes and the command line.
  *
  *      A closing rig closes local loops as one body, on the context's graph (T_x_i = T_x_0 * T_0i throughout):
  *        - on a fused frame after the rig's first (has_pose frames too), after step 3: each member's predict() ACTIVE at (time, time,
@@ -560,6 +565,8 @@ typedef struct {
                                                close_loops, icp_weight, pyramid, fast_odom and so3 */
   double T_0i[EF_MAX_CAMERAS][16];          /* row-major, camera i -> member 0's camera: rigid (|R^T R - I| <= 1e-6 entrywise, last row
                                                0 0 0 1, finite); T_0i[0] is the identity */
+  int32_t joint_so3;                        /* 0: member 0's SO(3) pre-alignment seeds the rig; 1 (members with so3 = 1): one joint
+                                               SO(3) pre-alignment over every member's image pair (see step 2) */
 } EfRigConfig;
 typedef struct {                            /* as EfCameraFrame, once for the rig */
   int32_t time;                             /* >= 0 */
@@ -577,7 +584,7 @@ typedef struct {
 } EfRigResult;
 /* EF_EINVAL for a NULL argument, n outside 1..EF_MAX_CAMERAS, a camera of another context or listed twice, one already in a rig, a
  * member with rgb_only set, members whose close_loops, icp_weight, pyramid, fast_odom or so3 differ, a T_0i that is not rigid or
- * finite, or T_0i[0] not the identity. EF_ENOMEM when a closing rig's buffers cannot be allocated (the context stays usable).
+ * finite, T_0i[0] not the identity, a joint_so3 other than 0 and 1, or joint_so3 = 1 with members whose so3 = 0. EF_ENOMEM when a closing rig's buffers cannot be allocated (the context stays usable).
  * Synchronises. */
 int ef_rig_create(EfContext* ctx, const EfRigConfig* cfg, EfRig** out);
 /* frees the rig; its cameras stay and may run alone again. EF_EINVAL for a rig of another context. Synchronises. */
@@ -585,7 +592,9 @@ int ef_rig_destroy(EfContext* ctx, EfRig* rig);
 /* HOST inputs rgb[i] (RGB8, W_i*H_i*3 B) and depth[i] (uint16 millimetres) of member i; members: n results, member i's stats and
  * covariance its own (member 0's lastA / lastb are the joint system's); synchronises. trace (HOST, may be NULL when max_trace = 0):
  * n blocks of max_trace records, member i's at trace + i * max_trace, one per iteration of a tracked frame (member 0's SO(3) records
- * first) with its own A_icp / A_rgb / b_icp / b_rgb, its own combined lastA / lastb and the joint result; n_trace (may be NULL): the
+ * first, or with joint_so3 every member's own: its A_so3 / b_so3 / so3_residual, the joint 3x3 system in lastA[0..8] / lastb[0..2]
+ * and the joint update in result[0..2], 0 on the iteration that stops the loop) with its own A_icp / A_rgb / b_icp / b_rgb, its own
+ * combined lastA / lastb and the joint result; n_trace (may be NULL): the
  * n record counts. EF_EINVAL for a NULL argument, a rig of another context, a negative time, a bad weight_multiplier, a non-finite
  * pose entry with has_pose, or a negative max_trace. */
 int ef_rig_frame(EfContext* ctx, EfRig* rig, const EfRigFrame* frame, const uint8_t* const* rgb, const uint16_t* const* depth,
